@@ -377,7 +377,9 @@ __global__ void __launch_bounds__(256) dsm_cell_kernel(const __grid_constant__ D
     double num = 0.0, den = 0.0;
     int cnt = 0;
     bool coincident = false;
-    unsigned long long match_idx = ~0ull;  // OrthoFromPcl: zero-distance point with the smallest id
+    // OrthoFromPcl: the zero-distance point with the LARGEST id, i.e. the last one the reference's loop would visit in
+    // point order (ortho-from-pcl.cc:90-96 keeps the last perfect match; its kd-tree order is not reproducible here)
+    long long match_idx = -1;
     double match_z = 0.0;
     for (int kj = kbj0; kj <= kbj1; ++kj) {
       const size_t row = static_cast<size_t>(kj) * plan.KR;
@@ -398,8 +400,8 @@ __global__ void __launch_bounds__(256) dsm_cell_kernel(const __grid_constant__ D
             den += w;
           } else {
             coincident = true;
-            const unsigned long long id = rec_id(__ldg(&pr->idx));
-            if (id < match_idx) {
+            const long long id = static_cast<long long>(rec_id(__ldg(&pr->idx)));
+            if (id > match_idx) {
               match_idx = id;
               match_z = pz;
             }
@@ -411,9 +413,9 @@ __global__ void __launch_bounds__(256) dsm_cell_kernel(const __grid_constant__ D
       num += __shfl_xor_sync(0xffffffffu, num, o);
       den += __shfl_xor_sync(0xffffffffu, den, o);
       cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-      const unsigned long long oi = __shfl_xor_sync(0xffffffffu, match_idx, o);
+      const long long oi = __shfl_xor_sync(0xffffffffu, match_idx, o);
       const double oz = __shfl_xor_sync(0xffffffffu, match_z, o);
-      if (oi < match_idx) {
+      if (oi > match_idx) {
         match_idx = oi;
         match_z = oz;
       }

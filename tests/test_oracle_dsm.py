@@ -151,3 +151,27 @@ def test_cell_range_sample_equals_full_run():
     assert st == 0
     assert np.array_equal(part[:, 10:25].view(np.uint32), full[:, 10:25].view(np.uint32))
     assert np.isnan(part[:, :10]).all() and np.isnan(part[:, 25:]).all()
+
+
+# ---- the probe scenes of tests/test_gpu_dsm_adversarial.py, on the oracle alone -----------------------------------------
+def test_the_half_integer_scenes_reach_the_last_window_row():
+    # the constructed points land in the last bin row half_widths() keeps (otherwise those scenes test nothing there)
+    import math
+    from common import last_window_row_hits, reach_scene
+    assert last_window_row_hits(reach_scene(1, 0.4)) > 0
+    assert last_window_row_hits(reach_scene(2, math.sqrt(2.0) / 3.5)) > 0
+
+
+@pytest.mark.parametrize("radius", [1, 2, 3])
+def test_probe_ties_decided_by_the_strict_threshold_like_brute_force(radius):
+    # exact ties at every retry level: the oracle's levels, counts and heights equal the brute-force definition's, and
+    # every probe gets the level and count the strict `<` implies for its d2
+    from common import tie_scene
+    sc = tie_scene(radius, 0.5)
+    st, e, cnt, lvl = _run(sc.rows, sc.cols, sc.res, sc.xyz, radius=radius)
+    assert st == 0
+    be, bc, bl = brute_dsm(sc.rows, sc.cols, sc.res, sc.xyz, radius)
+    assert np.array_equal(lvl, bl) and np.array_equal(cnt[bl >= 0], bc[bl >= 0])
+    assert ulp_diff(e, be).max() <= 1
+    for (i, j, level, count) in sc.probes:
+        assert lvl[i, j] == level and (level < 0 or cnt[i, j] == count), (i, j)

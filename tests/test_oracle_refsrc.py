@@ -107,6 +107,71 @@ def test_dsm_reference_sub_range_is_the_same_cells_of_the_full_run():
     assert np.isnan(p[:k0]).all() and np.isnan(p[k1:]).all()
 
 
+def _probe_scenes():
+    import math
+    import common as scenes
+    utm = dict(pos=scenes.UTM, ce=scenes.UTM_SHIFT[0], cn=scenes.UTM_SHIFT[1])
+    return {"ties_r1": lambda: scenes.tie_scene(1, 0.5),
+            "ties_r2": lambda: scenes.tie_scene(2, 0.5),
+            "ties_r3": lambda: scenes.tie_scene(3, 0.5),
+            "reach_0.4": lambda: scenes.reach_scene(1, 0.4),
+            "reach_half_2": lambda: scenes.reach_scene(2, math.sqrt(2.0) / 3.5),
+            "edges": lambda: scenes.bin_edge_scene(0.25),
+            "apron": lambda: scenes.apron_scene(0.5),
+            "band": lambda: scenes.band_scene()[0],
+            "utm_ties": lambda: scenes.tie_scene(1, 0.25, levels=[0, 1, 10, 20], require_exact=False, **utm),
+            "utm_reach": lambda: scenes.reach_scene(1, 0.1, **utm)}
+
+
+@pytest.mark.parametrize("scene", sorted(_probe_scenes()))
+def test_probe_scene_decisions_equal_the_reference_nanoflann(scene):
+    # the adversarial probe scenes of the GPU tests (exact ties at every retry level, half-integer window widths, bin
+    # edges, the apron, UTM coordinates): the bucket oracle's neighbour sets against the reference's own kd-tree and dsm.cc
+    sc = _probe_scenes()[scene]()
+    g = po.make_geometry(sc.rows, sc.cols, sc.res, sc.pos[0], sc.pos[1])
+    xyz = sc.xyz
+    e_src = _nan_layer(sc.rows, sc.cols)
+    st, _ = po.refsrc_dsm_process(g, e_src, xyz, sc.radius, sc.ce, sc.cn)
+    assert st == 0, po.refsrc_last_error()
+    e_nf, e_b = _nan_layer(sc.rows, sc.cols), _nan_layer(sc.rows, sc.cols)
+    st, cnt_nf, lvl_nf, _ = po.dsm_process(g, e_nf, xyz, sc.radius, sc.ce, sc.cn, debug=True, use_ref=True)
+    assert st == 0
+    st, cnt_b, lvl_b, _ = po.dsm_process(g, e_b, xyz, sc.radius, sc.ce, sc.cn, num_threads=2, debug=True)
+    assert st == 0
+    assert np.array_equal(e_src.view(np.uint32), e_nf.view(np.uint32))
+    assert np.array_equal(lvl_b, lvl_nf) and np.array_equal(cnt_b[lvl_b >= 0], cnt_nf[lvl_b >= 0])
+    assert ulp_diff(e_src, e_b).max() <= 1
+    for (i, j, level, count) in sc.probes:
+        assert lvl_nf[i, j] == level and (level < 0 or cnt_nf[i, j] == count), (i, j)
+
+
+def test_coincident_points_the_oracle_takes_the_last_the_reference_its_tree_order():
+    # ortho-from-pcl.cc:90-96 keeps the LAST zero-distance point its loop visits, in the kd-tree's traversal order.  The
+    # oracle (and the GPU) take the last in point order, i.e. the largest index: a documented divergence — the value is
+    # always one of the cluster's intensities, but not necessarily the same one
+    from common import coincident_members, coincident_scene
+    rows, cols, res, xyz, inten, cells = coincident_scene()
+    qx, qy = synth.grid_positions(rows, cols, res)
+    members = coincident_members(xyz, qx, qy, cells)
+    g = po.make_geometry(rows, cols, res)
+    a = np.full((rows, cols), 255.0, np.float32, order="F")
+    b, c = a.copy(order="F"), a.copy(order="F")
+    assert po.refsrc_ortho_from_pcl_process(g, a, xyz, inten, 2, False) == 0, po.refsrc_last_error()
+    assert po.ortho_from_pcl_process(g, b, xyz, inten, 2, False, use_ref=True) == 0
+    assert po.ortho_from_pcl_process(g, c, xyz, inten, 2, False, num_threads=2) == 0
+    assert np.array_equal(a.view(np.uint32), b.view(np.uint32))
+    differ = 0
+    for (i, j), m in zip(cells, members):
+        assert a[i, j] in set(np.float32(inten[m]).tolist())
+        assert c[i, j] == np.float32(inten[m.max()])
+        differ += a[i, j] != c[i, j]
+    assert differ >= 1                      # the divergence is real on this scene
+    other = np.ones((rows, cols), bool)
+    for (i, j) in cells:
+        other[i, j] = False
+    assert ulp_diff(a[other], c[other]).max() <= 1
+
+
 # ---- ortho-backward-grid.cc ------------------------------------------------------------------------------------
 def _scene(rows, cols, res, dist_type, dist, colored, seed, n_lines=2, per_line=3, agl=45.0, extrinsics=False):
     camd = synth.scaled_camera(0.05, dist_type=dist_type, dist=dist)

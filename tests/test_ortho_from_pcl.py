@@ -66,6 +66,22 @@ def test_oracle_equals_reference_nanoflann_and_perfect_match():
     assert po.ortho_from_pcl_process(g, c, np.zeros((0, 3)), np.zeros(0, np.int32)) == -1     # CHECK(!empty)
 
 
+def test_oracle_takes_the_last_coincident_point_in_point_order():
+    # several points exactly on one cell centre: ortho-from-pcl.cc:90-96 keeps the last perfect match its loop visits;
+    # the oracle's loop visits them in point order (one bucket, ascending index), so the largest index wins
+    rows, cols, res = 12, 10, 1.0
+    qx, qy = synth.grid_positions(rows, cols, res)
+    xyz, inten = make_cloud(30, 4.0, 3.0, 8)
+    for k in (3, 11, 17, 26):
+        xyz[k, :2] = (qx[5], qy[4])
+    inten[[3, 11, 17, 26]] = [9, 200, 31, 77]
+    o = np.full((rows, cols), 255.0, np.float32, order="F")
+    assert po.ortho_from_pcl_process(po.make_geometry(rows, cols, res), o, xyz, inten, radius=2) == 0
+    assert o[5, 4] == 77.0
+    b = brute(rows, cols, res, xyz, inten, 2, np.full((rows, cols), 255.0, np.float32, order="F"))
+    assert ulp_diff(o, b).max() <= 1
+
+
 @pytest.mark.gpu
 @pytest.mark.parametrize("rows,cols,res,n,radius,seed", [(120, 90, 0.5, 20000, 2, 3), (64, 64, 1.0, 3000, 10, 4),
                                                          (200, 150, 0.25, 9000, 1, 5)])
