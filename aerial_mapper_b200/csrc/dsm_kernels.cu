@@ -717,7 +717,7 @@ int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, 
   const bool f32 = ctx->dsm_precision == AMB_DSM_F32 && mode == 0;
   int f32_bps = 5;  // register-allocation target of the f32 gather (development knob: AMB_DSM_F32_BPS=4)
   if (const char* e = std::getenv("AMB_DSM_F32_BPS")) f32_bps = e[0] == '4' ? 4 : 5;
-  // f32: record 16 + original index 4 + record position 4 + 2 raw-record bin ids 2 x 2 + bin id of the slot 2
+  // f32: record 16 + original index in bin order 4 + compact list of the kept records (position 4, index 4, bin 2)
   const size_t per_point = f32 ? 16 + 4 + 4 + 2 * 2 + 2 : 16 + 8 + 4;
   if (f32) {  // bins of 1 x kStrip cells (dsm_gather_f32.inc): a much smaller start table
     const int NJb = (NJw + kStrip - 1) / kStrip;
