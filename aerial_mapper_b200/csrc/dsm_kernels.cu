@@ -9,23 +9,27 @@
 //
 // Layout of the work
 //   HBM:   points are sorted into COARSE buckets of BxB grid cells (B a power of two chosen so that a bucket holds
-//          a few dozen points; 8x8 cells at the benchmark density).  The bucket histogram is small enough to live
-//          in L2 (1.6 M counters at 10^4 x 10^4 cells), so counting and scattering do not pay a DRAM
-//          read-modify-write per point, and a bucket's records are one contiguous ~1 KB run.
-//   SMEM:  a 32x32-cell tile loads the buckets overlapping its window (tile + apron), bins their points to CELLS with
-//          shared-memory atomics, orders every cell's points by original index, and gathers from there.
+//          a few dozen points; 8x8 cells at the benchmark density), each bucket's records one contiguous run.  Every
+//          32-byte record {x, y, z, index word} carries the point's fine bin (nearest cell), computed once.
+//   SMEM:  a 32x32-cell tile loads the buckets overlapping its window (tile + apron), bins their points with
+//          shared-memory atomics, orders every bin's points by original index, and gathers from there.
 //
 // Pipeline (all on the context's stream):
-//   K1 dsm_count_kernel     AoS points -> bucket histogram (atomics resolve in L2)
-//   K2 scan_*               inclusive scan -> bucket start offsets
-//   K3 dsm_scatter_kernel   32-byte records {x, y, z, original index} into bucket order
-//   K3b dsm_bucket_order_kernel  one warp per bucket: visiting order of its records by original index (canonical
-//                           order: the IDW summation order — hence every output bit — is independent of atomic
-//                           scheduling and of how the map is striped across GPUs)
-//   K4 dsm_gather_kernel    one tile per block: bucket runs -> cell bins in shared memory -> every thread owns a
-//                           1x4 strip of cells and walks the strip's bin rows in one flattened, branch-free loop
-//   K5 dsm_cell_kernel      one warp per listed cell: cells whose primary ball is empty (expanding-radius retry,
-//                           dsm.cc:133-144) and all cells of tiles too dense for the shared-memory stage
+//   K1 dsm_partition_kernel      (dsm_partition.inc) bins every point once in double precision, counts the buckets
+//                                (atomics resolve in L2) and groups each tile of 2048 points by coarse destination
+//   K2 scan_*                    inclusive scan of the bucket counts -> bucket start offsets
+//   K3 dsm_fine_scatter_kernel   (dsm_partition.inc) records into bucket order, one coarse destination at a time
+//   K4 dsm_gather_kernel_f32     one tile per block: bucket runs -> bins in shared memory -> every thread owns a 1x4
+//      dsm_gather_kernel         strip of cells and walks the strip's bin rows in one flattened loop.  FP32 sums with
+//                                exact decisions (the default; Dsm only) or all FP64; cells it cannot decide exactly
+//                                and every cell of a tile too dense for the stage go to the cell list
+//   K5 dsm_mark_buckets_kernel   flags the buckets the listed cells can reach (Dsm; OrthoFromPcl orders every bucket
+//      dsm_bucket_order_kernel   after K3): the visiting order of a flagged bucket's records by original index
+//                                (canonical order: the IDW summation order — hence every output bit — is independent
+//                                of atomic scheduling and of how the map is striped across GPUs)
+//   K6 dsm_cell_kernel           one warp per listed cell: the expanding-radius retry (dsm.cc:133-144) and the cells
+//                                handed over by K4, from the bucket records in HBM
+// With amb_dsm_set_stream_chunks, K4-K6 run once per group of tile columns.
 //
 // Membership (d2 < threshold) is evaluated with __dmul_rn/__dadd_rn (no FMA contraction) in the reference's
 // operation order, so neighbour sets and retry levels are bit-exact decisions.  Heights differ from the CPU only
@@ -77,21 +81,6 @@ __device__ __forceinline__ void store_rec(PointRec* dst, double x, double y, dou
                : "memory");
 #endif
 }
-__device__ __forceinline__ void load_rec(const PointRec* src, double* x, double* y, double* z, double* idx_bits) {
-#ifdef AMB_CUDA_EMU
-  *x = src->x;
-  *y = src->y;
-  *z = src->z;
-  *idx_bits = __longlong_as_double(static_cast<long long>(src->idx));
-#else
-  asm volatile("ld.global.nc.v2.f64 {%0, %1}, [%4];\n\tld.global.nc.v2.f64 {%2, %3}, [%4+16];"
-               : "=d"(*x), "=d"(*y), "=d"(*z), "=d"(*idx_bits)
-               : "l"(src));
-#endif
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// K1: bucket histogram.  count(b) goes to G[b + 2] so that after the inclusive scan G[b + 1] = start(b).
 // Slot `s` of the gathered halos -> its record, or nullptr (own segment, beyond the segment's count).
 __device__ __forceinline__ const double* halo_record(const HaloSource& h, size_t s) {
   const unsigned int r = static_cast<unsigned int>(s / h.capacity);
@@ -195,7 +184,7 @@ __global__ void __launch_bounds__(256) scan_apply_kernel(uint4* __restrict__ dat
 // K1 / K3: two-level binning
 #include "dsm_partition.inc"
 
-// K3b: canonical order inside every bucket (ascending original index = what a stable sort would give), as an
+// K5: canonical order inside every bucket (ascending original index = what a stable sort would give), as an
 // index array: order[s + r] = position of the bucket's r-th smallest original index.  Only the warp-per-cell
 // kernel needs it (the tile kernel orders every cell's points in shared memory); writing 4 bytes per point
 // instead of permuting the 32-byte records keeps this pass at one read of the records.
@@ -284,21 +273,23 @@ __global__ void __launch_bounds__(256) dsm_mark_buckets_kernel(const __grid_cons
                                                                const unsigned int* __restrict__ counters,
                                                                unsigned char* __restrict__ flags) {
   const unsigned int n_cells = counters[CTR_DSM_LIST];
-  const int P = plan.P;
   for (unsigned int c = blockIdx.x * blockDim.x + threadIdx.x; c < n_cells; c += gridDim.x * blockDim.x) {
     const unsigned int cell = cell_list[c];
     const int i = static_cast<int>(cell % static_cast<unsigned int>(plan.rows));
     const int jl = static_cast<int>(cell / static_cast<unsigned int>(plan.rows));
-    const int bi = i + plan.Pa, bj = plan.col_begin + jl - plan.gj0;
-    const int kbi0 = max(bi - P, 0) >> plan.Bshift, kbi1 = min(bi + P, plan.BR - 1) >> plan.Bshift;
-    const int kbj0 = max(bj - P, 0) >> plan.Bshift, kbj1 = min(bj + P, plan.BC - 1) >> plan.Bshift;
-    for (int kj = kbj0; kj <= kbj1; ++kj)
-      for (int ki = kbi0; ki <= kbi1; ++ki) flags[static_cast<size_t>(kj) * plan.KR + ki] = 1;
+    const BucketWindow w = bucket_window(plan, i + plan.Pa, plan.col_begin + jl - plan.gj0, plan.P);
+    for (int kj = w.kbj0; kj <= w.kbj1; ++kj)
+      for (int ki = w.kbi0; ki <= w.kbi1; ++ki) flags[static_cast<size_t>(kj) * plan.KR + ki] = 1;
   }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// K4: tile gather
+// K4: tile gather, one block per TI x TJ tile: the records of the buckets overlapping the tile's window (the tile and W
+// cells around it) are staged in shared memory by bin, then every thread evaluates a 1 x kStrip strip of cells.  Two
+// kernels share the staging below: dsm_gather_kernel (dsm_gather_body.inc, all FP64, bins of one cell) and
+// dsm_gather_kernel_f32 (dsm_gather_f32.inc, FP32 sums, bins of 1 x kBinJ cells; the default).
+constexpr int kBinJ = kStrip;
+
 struct GatherArgs {
   const unsigned int* G;   // bucket starts
   const PointRec* rec;
@@ -311,11 +302,207 @@ struct GatherArgs {
   int tiles_i;
 };
 
+// Shared-memory carve of a gather block (byte offsets into the dynamic shared memory), used by dsm_run to size the stage
+// and by both kernels to place their arrays:
+//   A[N + 2] | srow[n_bin_rows] | run_pre[max_runs + 1] | run_g0[max_runs] | pad to 16 B |  capacity x per_point
+// A: per bin of the window, its count and then its start.  The staged points, FP64 (28 B): xy 16 | z 8 | original
+// index 4.  FP32 (30 B): {x, z - z0, y, y} 16 | original index in bin order 4 | pass 1's compact lists of the kept
+// records: HBM position 4 | original index 4 | bin 2.
+struct GatherCarve {
+  int NIw, NJw;    // window of the tile in cells
+  int bin_j;       // cells per bin along j
+  int N;           // bins of the window
+  int n_bin_rows;  // bin rows a strip's window spans (window row 0 is bin-aligned)
+  int srow, run_pre, run_g0;
+  int table_bytes, per_point;
+  int pts, z, sidx;     // z: FP64 only
+  int ksrc, kid, klin;  // FP32 only
+};
+__host__ __device__ inline GatherCarve gather_carve(int W, int B, bool f32, int capacity) {
+  GatherCarve c = {};
+  c.NIw = TI + 2 * W;
+  c.NJw = TJ + 2 * W;
+  c.bin_j = f32 ? kBinJ : 1;
+  c.N = c.NIw * ((c.NJw + c.bin_j - 1) / c.bin_j);
+  c.n_bin_rows = (kStrip + 2 * W + c.bin_j - 1) / c.bin_j;
+  const int max_runs = (c.NJw + B - 1) / B + 1;  // bucket rows overlapping the window
+  c.srow = 4 * (c.N + 2);
+  c.run_pre = c.srow + 4 * c.n_bin_rows;
+  c.run_g0 = c.run_pre + 4 * (max_runs + 1);
+  c.table_bytes = (c.run_g0 + 4 * max_runs + 15) & ~15;
+  c.pts = c.table_bytes;
+  if (f32) {
+    c.per_point = 16 + 4 + 4 + 4 + 2;
+    c.sidx = c.pts + 16 * capacity;
+    c.ksrc = c.sidx + 4 * capacity;
+    c.kid = c.ksrc + 4 * capacity;
+    c.klin = c.kid + 4 * capacity;
+  } else {
+    c.per_point = 16 + 8 + 4;
+    c.z = c.pts + 16 * capacity;
+    c.sidx = c.z + 8 * capacity;
+  }
+  return c;
+}
+
+// The block's tile, its window in fine bins and the buckets overlapping the window.
+struct GatherTile {
+  int i0;                        // first row of the tile
+  int gj;                        // global column of its first cell
+  int jl0;                       // slab-local column of its first cell (negative if the tile starts left of the stripe)
+  int wi0, wj0;                  // window origin in fine bins (>= 0: Pa >= W)
+  int kbi0, kbi1, kbj0, n_runs;  // buckets: rows kbj0 .. kbj0 + n_runs - 1, each over bucket columns kbi0 .. kbi1
+};
+__device__ __forceinline__ GatherTile gather_tile(const DsmPlan& plan, const GatherArgs& args, const GatherCarve& c) {
+  GatherTile t;
+  t.i0 = static_cast<int>(blockIdx.x % args.tiles_i) * TI;
+  t.gj = (plan.tile_j0 + static_cast<int>(blockIdx.x / args.tiles_i)) * TJ;
+  t.jl0 = t.gj - plan.col_begin;
+  t.wi0 = t.i0 + plan.Pa - plan.W;
+  t.wj0 = t.gj - plan.gj0 - plan.W;
+  t.kbi0 = t.wi0 >> plan.Bshift;
+  t.kbi1 = min(t.wi0 + c.NIw - 1, plan.BR - 1) >> plan.Bshift;
+  t.kbj0 = t.wj0 >> plan.Bshift;
+  t.n_runs = (min(t.wj0 + c.NJw - 1, plan.BC - 1) >> plan.Bshift) - t.kbj0 + 1;
+  return t;
+}
+
+// Tables of the tile (the caller's barrier publishes them):
+//   run_pre / run_g0: one contiguous record run per bucket row of the window; run q holds the window's raw records
+//     [run_pre[q], run_pre[q + 1]), starting at record run_g0[q].  Warp 0 fetches the bounds, one lane per bucket row,
+//     and prefix-sums the lengths with a shuffle scan (no serial chain of dependent global loads).
+//   srow[b]: half-width (in bins along i) of bin row b of a strip's window, the widest reach among its cell rows and the
+//     strip's cells; -1: out of reach.
+//   A: zeroed.
+__device__ __forceinline__ void gather_tables(const DsmPlan& plan, const GatherArgs& args, const GatherCarve& c,
+                                              const GatherTile& t) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  unsigned int* A = reinterpret_cast<unsigned int*>(smem_raw);
+  int* srow = reinterpret_cast<int*>(smem_raw + c.srow);
+  unsigned int* run_pre = reinterpret_cast<unsigned int*>(smem_raw + c.run_pre);
+  unsigned int* run_g0 = reinterpret_cast<unsigned int*>(smem_raw + c.run_g0);
+  if (threadIdx.x < 32) {
+    const int lane = threadIdx.x;
+    unsigned int carry = 0;
+    for (int r0 = 0; r0 < t.n_runs; r0 += 32) {
+      const int r = r0 + lane;
+      unsigned int g0 = 0, len = 0;
+      if (r < t.n_runs) {
+        const size_t row = static_cast<size_t>(t.kbj0 + r) * plan.KR;
+        g0 = __ldg(&args.G[row + t.kbi0]);
+        len = __ldg(&args.G[row + t.kbi1 + 1]) - g0;
+      }
+      unsigned int inc = len;
+      for (int o = 1; o < 32; o <<= 1) {
+        const unsigned int v = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc += v;
+      }
+      if (r < t.n_runs) {
+        run_pre[r] = carry + inc - len;
+        run_g0[r] = g0;
+      }
+      carry += __shfl_sync(0xffffffffu, inc, 31);
+    }
+    if (lane == 0) run_pre[t.n_runs] = carry;
+  }
+  for (int b = threadIdx.x; b < c.n_bin_rows; b += kGatherThreads) {
+    int hmax = -1;
+    for (int rr = 0; rr < c.bin_j; ++rr) {
+      const int r = b * c.bin_j + rr;  // cell row of the strip's window: (first cell's j) - W + r
+      for (int m = 0; m < kStrip; ++m) {
+        const int dj = r - plan.W - m;
+        const int ad = dj < 0 ? -dj : dj;
+        const int h = ad <= plan.W ? plan.hw[ad] : -1;
+        hmax = max(hmax, h);
+      }
+    }
+    srow[b] = hmax;
+  }
+  for (int e = threadIdx.x; e < c.N + 2; e += kGatherThreads) A[e] = 0;
+}
+
+// A raw record of the window: its position in HBM, its index word (PointRec::idx) and the window row of its bucket
+// row's first fine bin row.
+struct RawRecord {
+  unsigned int src;
+  int jrow;
+  unsigned long long word;
+};
+// Locates raw record `raw` (< run_pre[n_runs]) and reads its index word.  Runs are about equally long, so the search
+// starts at the proportional guess (raw * run_scale) >> 16, run_scale = (n_runs << 16) / n_in.  (Locating and binning
+// are two calls so that a caller can keep several loads in flight before it bins.)
+__device__ __forceinline__ RawRecord locate_record(const DsmPlan& plan, const GatherArgs& args, const GatherCarve& c,
+                                                   const GatherTile& t, unsigned int run_scale, unsigned int raw) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const unsigned int* run_pre = reinterpret_cast<const unsigned int*>(smem_raw + c.run_pre);
+  const unsigned int* run_g0 = reinterpret_cast<const unsigned int*>(smem_raw + c.run_g0);
+  int run = min(static_cast<int>((raw * run_scale) >> 16), t.n_runs - 1);
+  while (raw < run_pre[run]) --run;
+  while (raw >= run_pre[run + 1]) ++run;
+  RawRecord r;
+  r.src = run_g0[run] + (raw - run_pre[run]);
+  r.jrow = ((t.kbj0 + run) << plan.Bshift) - t.wj0;
+  r.word = __ldg(&args.rec[r.src].idx);
+  return r;
+}
+// Bin of the window a located record falls in, or -1 outside the window.  The binning stored the point's fine bin
+// (fine_bin(), double precision) in the index word, so only integer arithmetic is left: bi = code >> 4, and bj's low
+// bits are code & (B - 1) on top of the bucket row's first fine bin row.
+__device__ __forceinline__ int record_bin(const DsmPlan& plan, const GatherCarve& c, const GatherTile& t,
+                                          const RawRecord& r) {
+  const unsigned int code = rec_code(r.word);
+  const int ii = static_cast<int>(code >> 4) - t.wi0;
+  const int jj = r.jrow + static_cast<int>(code & static_cast<unsigned int>(plan.B - 1));
+  return ii >= 0 && ii < c.NIw && jj >= 0 && jj < c.NJw ? (jj / c.bin_j) * c.NIw + ii : -1;
+}
+
+// x, y, z of a record without its index word
+__device__ __forceinline__ void load_xyz(const PointRec* src, double* x, double* y, double* z) {
+#ifdef AMB_CUDA_EMU
+  *x = src->x;
+  *y = src->y;
+  *z = src->z;
+#else
+  asm volatile("ld.global.nc.v2.f64 {%0, %1}, [%3];\n\tld.global.nc.f64 %2, [%3+16];"
+               : "=d"(*x), "=d"(*y), "=d"(*z)
+               : "l"(src));
+#endif
+}
+
+// In-place inclusive scan of A[0 .. n) (thread t owns a contiguous chunk), then a barrier.
+__device__ __forceinline__ void scan_bins(unsigned int* A, int n) {
+  __shared__ unsigned int total;
+  const int per = (n + kGatherThreads - 1) / kGatherThreads;
+  const int lo = min(static_cast<int>(threadIdx.x) * per, n), hi = min(lo + per, n);
+  unsigned int s = 0;
+  for (int e = lo; e < hi; ++e) s += A[e];
+  unsigned int run = block_exclusive_scan(s, &total);
+  for (int e = lo; e < hi; ++e) {
+    run += A[e];
+    A[e] = run;
+  }
+  __syncthreads();
+}
+
+// Every cell of the tile goes to the warp-per-cell kernel (dense tile, non-finite heights ...).  The decision depends
+// only on the point set the tile stages, which is the same for every striping of the map (tiles align to global
+// columns, amb_dsm_halo_reach covers whole tile windows).
+__device__ __forceinline__ void tile_to_cell_list(const DsmPlan& plan, const GatherArgs& args, const GatherTile& t) {
+  if (threadIdx.x == 0) atomicAdd(&args.counters[CTR_DSM_DENSE], 1u);
+  const int ti = threadIdx.x & 31, tq = threadIdx.x >> 5;
+  for (int m = 0; m < kStrip; ++m) {
+    const int i = t.i0 + ti, jl = t.jl0 + kStrip * tq + m;
+    const bool valid = i < plan.rows && jl >= 0 && jl < plan.cols_slab;
+    warp_append(valid, &args.counters[CTR_DSM_LIST], args.cell_list,
+                static_cast<unsigned int>(static_cast<size_t>(jl) * plan.rows + i));
+  }
+}
+
 #include "dsm_gather_body.inc"
 #include "dsm_gather_f32.inc"
 
 // ---------------------------------------------------------------------------------------------------------------
-// K5: one warp per listed cell.  Evaluates the reference's complete per-cell sequence (primary query, then the
+// K6: one warp per listed cell.  Evaluates the reference's complete per-cell sequence (primary query, then the
 // expanding-radius retry dsm.cc:133-144) from the bucket records in HBM: cells left empty by the tile kernel and
 // every cell of a tile too dense for the shared-memory stage.
 struct CellArgs {
@@ -333,7 +520,6 @@ __global__ void __launch_bounds__(256) dsm_cell_kernel(const __grid_constant__ D
   const int lane = threadIdx.x & 31;
   const unsigned int n_cells = args.counters[CTR_DSM_LIST];
   const unsigned int warps_total = gridDim.x * (blockDim.x >> 5);
-  const int P = plan.P;
   for (unsigned int c = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); c < n_cells; c += warps_total) {
     const unsigned int cell = args.cell_list[c];
     const int i = static_cast<int>(cell % static_cast<unsigned int>(plan.rows));
@@ -341,23 +527,8 @@ __global__ void __launch_bounds__(256) dsm_cell_kernel(const __grid_constant__ D
     const double qx = cell_x(plan, i);
     const double qy = cell_y(plan, plan.col_begin + jl);
     // buckets overlapping the window of the largest threshold (fine bins [b - P, b + P] on both axes)
-    const int bi = i + plan.Pa, bj = plan.col_begin + jl - plan.gj0;
-    const int kbi0 = max(bi - P, 0) >> plan.Bshift, kbi1 = min(bi + P, plan.BR - 1) >> plan.Bshift;
-    const int kbj0 = max(bj - P, 0) >> plan.Bshift, kbj1 = min(bj + P, plan.BC - 1) >> plan.Bshift;
-    // pass 1: smallest d2
-    double dmin = DBL_MAX;
-    for (int kj = kbj0; kj <= kbj1; ++kj) {
-      const size_t row = static_cast<size_t>(kj) * plan.KR;
-      const unsigned int a = args.G[row + kbi0];
-      const unsigned int b = args.G[row + kbi1 + 1];
-      for (unsigned int k = a + lane; k < b; k += 32) {  // min is order-independent: no indirection needed
-        const double2 v = __ldg(reinterpret_cast<const double2*>(args.rec + k));
-        const double dx = qx - v.x;
-        const double dy = qy - v.y;
-        dmin = fmin(dmin, __dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)));
-      }
-    }
-    for (int o = 16; o > 0; o >>= 1) dmin = fmin(dmin, __shfl_xor_sync(0xffffffffu, dmin, o));
+    const BucketWindow w = bucket_window(plan, i + plan.Pa, plan.col_begin + jl - plan.gj0, plan.P);
+    const double dmin = window_min_d2(plan, args.G, args.rec, w, qx, qy, lane);
     // first threshold whose (strict) ball is non-empty: k = 0 is the primary query itself
     int level = -1;
     for (int k = 0; k < plan.n_thr; ++k) {
@@ -381,10 +552,10 @@ __global__ void __launch_bounds__(256) dsm_cell_kernel(const __grid_constant__ D
     // point order (ortho-from-pcl.cc:90-96 keeps the last perfect match; its kd-tree order is not reproducible here)
     long long match_idx = -1;
     double match_z = 0.0;
-    for (int kj = kbj0; kj <= kbj1; ++kj) {
+    for (int kj = w.kbj0; kj <= w.kbj1; ++kj) {
       const size_t row = static_cast<size_t>(kj) * plan.KR;
-      const unsigned int a = args.G[row + kbi0];
-      const unsigned int b = args.G[row + kbi1 + 1];
+      const unsigned int a = args.G[row + w.kbi0];
+      const unsigned int b = args.G[row + w.kbi1 + 1];
       for (unsigned int k = a + lane; k < b; k += 32) {
         const PointRec* pr = args.rec + __ldg(args.order + k);  // canonical order: lane partial sums are fixed
         const double2 v = __ldg(reinterpret_cast<const double2*>(pr));
@@ -708,22 +879,10 @@ int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, 
   AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_BIN_END], s));
 
   // gather
-  const int W = plan.W;
-  const int NIw = TI + 2 * W, NJw = TJ + 2 * W;
-  const int max_runs = (NJw + B - 1) / B + 1;
-  size_t off_bytes = (static_cast<size_t>(NIw) * NJw + 2 + kStrip + 2 * W + 2 * max_runs + 1) * 4;
-  off_bytes = (off_bytes + 15) & ~static_cast<size_t>(15);
   // FP32 gather (the default; amb_dsm_set_precision): Dsm only — OrthoFromPcl keeps the all-FP64 kernel
   const bool f32 = ctx->dsm_precision == AMB_DSM_F32 && mode == 0;
-  int f32_bps = 5;  // register-allocation target of the f32 gather (development knob: AMB_DSM_F32_BPS=4)
-  if (const char* e = std::getenv("AMB_DSM_F32_BPS")) f32_bps = e[0] == '4' ? 4 : 5;
-  // f32: record 16 + original index in bin order 4 + compact list of the kept records (position 4, index 4, bin 2)
-  const size_t per_point = f32 ? 16 + 4 + 4 + 2 * 2 + 2 : 16 + 8 + 4;
-  if (f32) {  // bins of 1 x kStrip cells (dsm_gather_f32.inc): a much smaller start table
-    const int NJb = (NJw + kStrip - 1) / kStrip;
-    off_bytes = (static_cast<size_t>(NIw) * NJb + 2 + (kStrip + 2 * W + kStrip - 1) / kStrip + 2 * max_runs + 1) * 4;
-    off_bytes = (off_bytes + 15) & ~static_cast<size_t>(15);
-  }
+  const GatherCarve carve = gather_carve(plan.W, B, f32, 0);
+  const size_t off_bytes = static_cast<size_t>(carve.table_bytes), per_point = static_cast<size_t>(carve.per_point);
   {
     // Bound on |d2_f32 - d2| (dsm_gather_f32.inc): local coordinates |c| <= M are rounded to float (relative u = 2^-24),
     // the difference adds one rounding, the two squares and the sum three more:
@@ -741,12 +900,14 @@ int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, 
   // Poisson count is far inside that; denser tiles go to the warp-per-cell kernel), clamped to [24 KB, 100 KB]
   // so that several blocks stay resident per SM (227 KB usable).
   if (off_bytes + per_point * 64 > 200 * 1024) return AMB_ERR_UNSUPPORTED;
-  const double expect = per_cell * static_cast<double>(NIw) * static_cast<double>(NJw);
+  const double expect = per_cell * static_cast<double>(carve.NIw) * static_cast<double>(carve.NJw);
   size_t smem = off_bytes + static_cast<size_t>((f32 ? 1.4 : 1.6) * expect + 64.0) * per_point;
   smem = std::min<size_t>(std::max<size_t>(smem, 24 * 1024), 100 * 1024);
   smem = std::max(smem, off_bytes + per_point * 64);
   smem = (smem + 1023) & ~static_cast<size_t>(1023);
   const int capacity = static_cast<int>((smem - off_bytes) / per_point) & ~1;
+  void (*const gather)(DsmPlan, GatherArgs) = f32 ? dsm_gather_kernel_f32 : dsm_gather_kernel;
+  AMB_CUDA(ctx, cudaFuncSetAttribute(gather, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   GatherArgs ga;
   ga.G = G;
   ga.rec = rec;
@@ -757,97 +918,54 @@ int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, 
   ga.dbg_level = ctx->dsm_debug ? ctx->dbg_level.as<signed char>() : nullptr;
   ga.capacity = capacity;
   ga.tiles_i = (plan.rows + TI - 1) / TI;
+  CellArgs ca;
+  ca.G = G;
+  ca.order = ctx->point_order.as<unsigned int>();
+  ca.rec = rec;
+  ca.elevation = ga.elevation;
+  ca.cell_list = ga.cell_list;
+  ca.counters = counters;
+  ca.dbg_count = ga.dbg_count;
+  ca.dbg_level = ga.dbg_level;
   const int tiles_j = tile_j1 - plan.tile_j0 + 1;
   // Opt-in chunking (amb_dsm_set_stream_chunks, only with a registered host mirror): the tile columns are evaluated in K
   // groups — gather + warp-per-cell fill per group — and each group's finished columns start travelling to the host
   // at once, so the download of the layer overlaps the evaluation of the remaining groups.  The launches of a group are
   // the un-chunked ones restricted to its tile columns (plan.tile_j0 and the grid size), so every result is unchanged.
   // (Dsm only: OrthoFromPcl's adaptive pass rewrites the layer afterwards, so its columns are not final per chunk)
+  // Without chunking the whole stripe is one group.
   const int chunks = (mode == 0 && ctx->dsm_stream_chunks > 1 && ctx->host_mirror[out_layer])
                          ? std::min(ctx->dsm_stream_chunks, tiles_j) : 1;
-  if (chunks > 1) {
-    AMB_CUDA(ctx, cudaFuncSetAttribute(dsm_gather_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       static_cast<int>(smem)));
-    AMB_CUDA(ctx, cudaFuncSetAttribute(dsm_gather_kernel_f32<4>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       static_cast<int>(smem)));
-    AMB_CUDA(ctx, cudaFuncSetAttribute(dsm_gather_kernel_f32<5>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       static_cast<int>(smem)));
-    CellArgs ca;
-    ca.G = G;
-    ca.order = ctx->point_order.as<unsigned int>();
-    ca.rec = rec;
-    ca.elevation = ga.elevation;
-    ca.cell_list = ga.cell_list;
-    ca.counters = counters;
-    ca.dbg_count = ga.dbg_count;
-    ca.dbg_level = ga.dbg_level;
-    for (int c = 0; c < chunks; ++c) {
-      const int tj0 = static_cast<int>(static_cast<long long>(tiles_j) * c / chunks);
-      const int tj1 = static_cast<int>(static_cast<long long>(tiles_j) * (c + 1) / chunks);
-      if (tj1 <= tj0) continue;
-      DsmPlan pc = plan;
-      pc.tile_j0 = plan.tile_j0 + tj0;
-      if (c > 0) roll_list_counter_kernel<<<1, 1, 0, s>>>(counters);  // the cell list restarts; its length is kept
-      if (f32 && f32_bps == 4) {
-        dsm_gather_kernel_f32<4><<<ga.tiles_i * (tj1 - tj0), kGatherThreads, smem, s>>>(pc, ga);
-      } else if (f32) {
-        dsm_gather_kernel_f32<5><<<ga.tiles_i * (tj1 - tj0), kGatherThreads, smem, s>>>(pc, ga);
-      } else {
-        dsm_gather_kernel<<<ga.tiles_i * (tj1 - tj0), kGatherThreads, smem, s>>>(pc, ga);
-      }
-      if (mode == 0) {
-        dsm_mark_buckets_kernel<<<ctx->num_sms * 2, 256, 0, s>>>(pc, ga.cell_list, counters, bucket_flags);
-        dsm_bucket_order_kernel<<<stream_grid, 256, 0, s>>>(G, static_cast<unsigned int>(nbk), rec,
-                                                            ctx->point_order.as<unsigned int>(), bucket_flags);
-        ctx->dsm_launches += 2;
-      }
-      dsm_cell_kernel<<<ctx->num_sms * 8, 256, 0, s>>>(pc, ca);
+  for (int c = 0; c < chunks; ++c) {
+    const int tj0 = static_cast<int>(static_cast<long long>(tiles_j) * c / chunks);
+    const int tj1 = static_cast<int>(static_cast<long long>(tiles_j) * (c + 1) / chunks);
+    if (tj1 <= tj0) continue;
+    DsmPlan pc = plan;
+    pc.tile_j0 = plan.tile_j0 + tj0;
+    if (c > 0) roll_list_counter_kernel<<<1, 1, 0, s>>>(counters);  // the cell list restarts; its length is kept
+    gather<<<ga.tiles_i * (tj1 - tj0), kGatherThreads, smem, s>>>(pc, ga);
+    if (chunks == 1) AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_GATHER_END], s));
+    if (mode == 0) {
+      dsm_mark_buckets_kernel<<<ctx->num_sms * 2, 256, 0, s>>>(pc, ga.cell_list, counters, bucket_flags);
+      dsm_bucket_order_kernel<<<stream_grid, 256, 0, s>>>(G, static_cast<unsigned int>(nbk), rec,
+                                                          ctx->point_order.as<unsigned int>(), bucket_flags);
       ctx->dsm_launches += 2;
+    }
+    dsm_cell_kernel<<<ctx->num_sms * 8, 256, 0, s>>>(pc, ca);
+    ctx->dsm_launches += 2;
+    if (chunks > 1) {
       // slab-local columns of this group's tiles (tiles are aligned to GLOBAL columns)
       const int col0 = std::max((plan.tile_j0 + tj0) * TJ - ctx->col_begin, 0);
       const int col1 = std::min((plan.tile_j0 + tj1) * TJ - ctx->col_begin, ctx->col_end - ctx->col_begin);
       st = mirror_layer_columns(ctx, out_layer, col0, col1);
       if (st != AMB_OK) return st;
     }
-    AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_GATHER_END], s));  // (stage split not meaningful when chunked)
-    AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_FILL_END], s));
-    AMB_CUDA(ctx, cudaGetLastError());
-  } else {
-    if (f32 && f32_bps == 4) {
-      AMB_CUDA(ctx, cudaFuncSetAttribute(dsm_gather_kernel_f32<4>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         static_cast<int>(smem)));
-      dsm_gather_kernel_f32<4><<<ga.tiles_i * tiles_j, kGatherThreads, smem, s>>>(plan, ga);
-    } else if (f32) {
-      AMB_CUDA(ctx, cudaFuncSetAttribute(dsm_gather_kernel_f32<5>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         static_cast<int>(smem)));
-      dsm_gather_kernel_f32<5><<<ga.tiles_i * tiles_j, kGatherThreads, smem, s>>>(plan, ga);
-    } else {
-      AMB_CUDA(ctx, cudaFuncSetAttribute(dsm_gather_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         static_cast<int>(smem)));
-      dsm_gather_kernel<<<ga.tiles_i * tiles_j, kGatherThreads, smem, s>>>(plan, ga);
-    }
-    ctx->dsm_launches += 1;
-    AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_GATHER_END], s));
-
-    CellArgs ca;
-    ca.G = G;
-    ca.order = ctx->point_order.as<unsigned int>();
-    ca.rec = rec;
-    ca.elevation = ga.elevation;
-    ca.cell_list = ga.cell_list;
-    ca.counters = counters;
-    ca.dbg_count = ga.dbg_count;
-    ca.dbg_level = ga.dbg_level;
-    if (mode == 0) {
-      dsm_mark_buckets_kernel<<<ctx->num_sms * 2, 256, 0, s>>>(plan, ga.cell_list, counters, bucket_flags);
-      dsm_bucket_order_kernel<<<stream_grid, 256, 0, s>>>(G, static_cast<unsigned int>(nbk), rec,
-                                                          ctx->point_order.as<unsigned int>(), bucket_flags);
-      ctx->dsm_launches += 2;
-    }
-    dsm_cell_kernel<<<ctx->num_sms * 8, 256, 0, s>>>(plan, ca);
-    ctx->dsm_launches += 1;
-    AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_FILL_END], s));
-    AMB_CUDA(ctx, cudaGetLastError());
+  }
+  // chunked: the stage split is not meaningful, both events mark the end
+  if (chunks > 1) AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_GATHER_END], s));
+  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_FILL_END], s));
+  AMB_CUDA(ctx, cudaGetLastError());
+  if (chunks == 1) {
     st = mirror_layer(ctx, out_layer);  // the result starts streaming to its host mirror (if one is registered)
     if (st != AMB_OK) return st;
   }

@@ -1,10 +1,13 @@
-// dsm_plan.h — the launch plan, the sorted-point record and the exact-arithmetic device helpers shared by the DSM
-// kernels (dsm_kernels.cu) and the adaptive OrthoFromPcl pass (pcl_adaptive_kernels.cu).
+// dsm_plan.h — the launch plan, the sorted-point record, the exact-arithmetic and bucket-window device helpers and the
+// warp-aggregated append shared by the DSM kernels (dsm_kernels.cu) and the adaptive OrthoFromPcl pass
+// (pcl_adaptive_kernels.cu).
 #ifndef AMB_DSM_PLAN_H_
 #define AMB_DSM_PLAN_H_
 
 #include <cuda_runtime.h>
 
+#include <cfloat>
+#include <cstddef>
 namespace amb {
 namespace dsmk {
 
@@ -68,6 +71,50 @@ __device__ __forceinline__ bool fine_bin(const DsmPlan& p, double px, double py,
   *bi = static_cast<int>(fi);
   *bj = static_cast<int>(fj);
   return true;
+}
+
+// Buckets overlapping fine bins [bi - P, bi + P] x [bj - P, bj + P] (clamped to the bin grid).  Bucket row kj of the
+// window is one contiguous record range, [G[kj * KR + kbi0], G[kj * KR + kbi1 + 1]).
+struct BucketWindow {
+  int kbi0, kbi1, kbj0, kbj1;
+};
+__device__ __forceinline__ BucketWindow bucket_window(const DsmPlan& p, int bi, int bj, int P) {
+  return {max(bi - P, 0) >> p.Bshift, min(bi + P, p.BR - 1) >> p.Bshift, max(bj - P, 0) >> p.Bshift,
+          min(bj + P, p.BC - 1) >> p.Bshift};
+}
+
+// Smallest d2 from (qx, qy) to the records of a bucket window, reduced over the warp (every lane calls it).  The minimum
+// does not depend on the visiting order, so the records are read in bucket order.
+__device__ __forceinline__ double window_min_d2(const DsmPlan& p, const unsigned int* G, const PointRec* rec,
+                                                const BucketWindow& w, double qx, double qy, int lane) {
+  double dmin = DBL_MAX;
+  for (int kj = w.kbj0; kj <= w.kbj1; ++kj) {
+    const size_t row = static_cast<size_t>(kj) * p.KR;
+    const unsigned int lo = G[row + w.kbi0];
+    const unsigned int hi = G[row + w.kbi1 + 1];
+    for (unsigned int k = lo + lane; k < hi; k += 32) {
+      const double2 v = __ldg(reinterpret_cast<const double2*>(rec + k));
+      const double dx = qx - v.x;
+      const double dy = qy - v.y;
+      dmin = fmin(dmin, __dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)));  // L2_Adaptor, un-contracted
+    }
+  }
+  for (int o = 16; o > 0; o >>= 1) dmin = fmin(dmin, __shfl_xor_sync(0xffffffffu, dmin, o));
+  return dmin;
+}
+
+// Warp-aggregated append: every lane of the warp calls it; the lanes with `take` store `value` to consecutive slots of
+// `list` in lane order, reserved by one atomic on `*counter`.
+__device__ __forceinline__ void warp_append(bool take, unsigned int* counter, unsigned int* list, unsigned int value) {
+  const unsigned int mask = __ballot_sync(0xffffffffu, take);
+  if (mask) {
+    const int lane = threadIdx.x & 31;
+    const int leader = __ffs(mask) - 1;
+    unsigned int base = 0;
+    if (lane == leader) base = atomicAdd(counter, static_cast<unsigned int>(__popc(mask)));
+    base = __shfl_sync(0xffffffffu, base, leader);
+    if (take) list[base + __popc(mask & ((1u << lane) - 1u))] = value;
+  }
 }
 
 // Reciprocal of a positive normal double to ~1 ulp: MUFU.RCP64H seed (rcp.approx.ftz.f64) + one cubic correction

@@ -50,42 +50,13 @@ struct AdaptiveArgs {
 __global__ void __launch_bounds__(256) pcl_adaptive_list_kernel(const float* __restrict__ ortho, size_t cells,
                                                                 unsigned int* __restrict__ cell_list,
                                                                 unsigned int* __restrict__ n_cells) {
-  const int lane = threadIdx.x & 31;
   // whole warps iterate together (the ballot needs every lane): round the trip count up to a warp multiple
   const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
   const size_t cells_up = (cells + 31) & ~static_cast<size_t>(31);
   for (size_t c = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; c < cells_up; c += stride) {
     const bool empty = c < cells && ortho[c] != ortho[c];  // still the NaN sentinel
-    const unsigned int mask = __ballot_sync(0xffffffffu, empty);
-    if (mask) {
-      const int leader = __ffs(mask) - 1;
-      unsigned int base = 0;
-      if (lane == leader) base = atomicAdd(n_cells, static_cast<unsigned int>(__popc(mask)));
-      base = __shfl_sync(0xffffffffu, base, leader);
-      if (empty) cell_list[base + __popc(mask & ((1u << lane) - 1u))] = static_cast<unsigned int>(c);
-    }
+    warp_append(empty, n_cells, cell_list, static_cast<unsigned int>(c));
   }
-}
-
-// Smallest d2 from (qx, qy) to the records of the buckets overlapping fine bins [bi - P, bi + P] x [bj - P, bj + P].
-__device__ __forceinline__ double window_min_d2(const DsmPlan& plan, const AdaptiveArgs& a, int lane, double qx,
-                                                double qy, int bi, int bj, int P) {
-  const int kbi0 = max(bi - P, 0) >> plan.Bshift, kbi1 = min(bi + P, plan.BR - 1) >> plan.Bshift;
-  const int kbj0 = max(bj - P, 0) >> plan.Bshift, kbj1 = min(bj + P, plan.BC - 1) >> plan.Bshift;
-  double dmin = DBL_MAX;
-  for (int kj = kbj0; kj <= kbj1; ++kj) {
-    const size_t row = static_cast<size_t>(kj) * plan.KR;
-    const unsigned int lo = a.G[row + kbi0];
-    const unsigned int hi = a.G[row + kbi1 + 1];
-    for (unsigned int k = lo + lane; k < hi; k += 32) {
-      const double2 v = __ldg(reinterpret_cast<const double2*>(a.rec + k));
-      const double dx = qx - v.x;
-      const double dy = qy - v.y;
-      dmin = fmin(dmin, __dadd_rn(__dmul_rn(dx, dx), __dmul_rn(dy, dy)));  // L2_Adaptor, un-contracted
-    }
-  }
-  for (int o = 16; o > 0; o >>= 1) dmin = fmin(dmin, __shfl_xor_sync(0xffffffffu, dmin, o));
-  return dmin;
 }
 
 __global__ void __launch_bounds__(256) pcl_adaptive_cell_kernel(const __grid_constant__ DsmPlan plan,
@@ -105,7 +76,7 @@ __global__ void __launch_bounds__(256) pcl_adaptive_cell_kernel(const __grid_con
     int level = -1;
     for (int L = 0; L < a.n_levels; ++L) {
       const int P = a.reach[L];
-      const double dmin = window_min_d2(plan, a, lane, qx, qy, bi, bj, P);
+      const double dmin = window_min_d2(plan, a.G, a.rec, bucket_window(plan, bi, bj, P), qx, qy, lane);
       if (dmin < a.thr[L]) {
         level = L;
         break;
@@ -127,14 +98,12 @@ __global__ void __launch_bounds__(256) pcl_adaptive_cell_kernel(const __grid_con
     }
 
     const double thr = a.thr[level];
-    const int P = a.reach[level];
-    const int kbi0 = max(bi - P, 0) >> plan.Bshift, kbi1 = min(bi + P, plan.BR - 1) >> plan.Bshift;
-    const int kbj0 = max(bj - P, 0) >> plan.Bshift, kbj1 = min(bj + P, plan.BC - 1) >> plan.Bshift;
+    const BucketWindow w = bucket_window(plan, bi, bj, a.reach[level]);
     double num = 0.0, den = 0.0;
-    for (int kj = kbj0; kj <= kbj1; ++kj) {
+    for (int kj = w.kbj0; kj <= w.kbj1; ++kj) {
       const size_t row = static_cast<size_t>(kj) * plan.KR;
-      const unsigned int lo = a.G[row + kbi0];
-      const unsigned int hi = a.G[row + kbi1 + 1];
+      const unsigned int lo = a.G[row + w.kbi0];
+      const unsigned int hi = a.G[row + w.kbi1 + 1];
       for (unsigned int k = lo + lane; k < hi; k += 32) {
         const PointRec* pr = a.rec + __ldg(a.order + k);  // canonical order: the lanes' partial sums are fixed
         const double2 v = __ldg(reinterpret_cast<const double2*>(pr));

@@ -11,12 +11,9 @@ that follow from the strict `<` for the d2 it actually got.
 Every DSM scene runs in both gather precisions and in every production variant:
   debug run        neighbour counts, levels and NaN mask equal to the oracle, heights within MAX_ULP;
   debug off        the production template (ROWS3 when a strip spans <= 3 bin rows)      -- bit-identical to the debug run
-  AMB_DSM_F32_BPS=4 the other register-allocation instantiation                            -- bit-identical
   chunked          pinned map with host mirrors: the column groups of amb_dsm_set_stream_chunks -- bit-identical
 The case 1 / 2 / 5 scenes are also compared with the reference's own dsm.cc (common.reference_outputs)."""
-import contextlib
 import math
-import os
 
 import numpy as np
 import pytest
@@ -35,22 +32,6 @@ MAX_ULP = {"f64": 1, "f32": 4}
 
 
 # ---- running ----------------------------------------------------------------------------------------------------------
-@contextlib.contextmanager
-def env(name, value):
-    old = os.environ.get(name)
-    if value is None:
-        os.environ.pop(name, None)
-    else:
-        os.environ[name] = value
-    try:
-        yield
-    finally:
-        if old is None:
-            os.environ.pop(name, None)
-        else:
-            os.environ[name] = old
-
-
 def gpu_run(sc, precision, xyz=None, debug=False, chunked=False, col_range=None):
     xyz = sc.xyz if xyz is None else xyz
     s = amb.GridMapSettings(sc.pos[0], sc.pos[1], sc.rows * sc.res, sc.cols * sc.res, sc.res)
@@ -96,9 +77,6 @@ def check_all_variants(sc, precision):
     bits = ge.view(np.uint32)
     prod, _, _ = gpu_run(sc, precision)
     assert np.array_equal(prod.view(np.uint32), bits), "production gather differs from the debug run"
-    with env("AMB_DSM_F32_BPS", "4"):
-        b4, _, _ = gpu_run(sc, precision)
-    assert np.array_equal(b4.view(np.uint32), bits), "AMB_DSM_F32_BPS=4 differs from the debug run"
     ch, _, _ = gpu_run(sc, precision, chunked=True)
     assert np.array_equal(ch.view(np.uint32), bits), "chunked evaluation differs from the debug run"
     return e, t
