@@ -210,7 +210,7 @@ struct amb_ctx {
   int64_t ortho_h2d_bytes = 0;
   bool ortho_two_phase = false;
   bool ortho_brute_force = false;
-  bool ortho_dominance = true;   // per-tile dominance cull of the frame list (ortho_kernel_dom); amb_ortho_set_dominance_cull(0) = plain list
+  bool ortho_dominance = true;   // per-tile dominance cull of the frame list (OrthoArgs::dominance); amb_ortho_set_dominance_cull(0) = plain list
 
   size_t slab_cells() const { return static_cast<size_t>(geom.rows) * static_cast<size_t>(col_end - col_begin); }
 };

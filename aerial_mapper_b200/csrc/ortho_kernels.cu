@@ -80,15 +80,13 @@ struct OrthoArgs {
   double fu, fv, cu, cv;
   double d0, d1, d2, d3;
   double cos_c, sin_c;            // half-angle of the conservative view cone
-  // --- dominance cull (DOM instances only; appended so that every earlier field keeps its offset) ---
-  // every ray with undistorted normalised keypoint inside [ui_lo, ui_hi] x [vi_lo, vi_hi] (and z_c > 0) IS visible
+  // dominance cull, rect: every ray with undistorted normalised keypoint inside [ui_lo, ui_hi] x [vi_lo, vi_hi] (and
+  // z_c > 0) IS visible
   double ui_lo, ui_hi, vi_lo, vi_hi;
   double nui_lo, nui_hi, nvi_lo, nvi_hi;  // sqrt(1 + bound^2)
-  double dom_margin;                      // rad
-  double dom_theta_in;                    // equidistant: every ray with angle-to-axis below this is imaged (else unused)
-  double dom_cos_in;                      // cos(dom_theta_in)
-  double dom_cos_margin, dom_sin_margin;  // cos / sin of dom_margin
-  // --- exact re-evaluation (appended) ---
+  double dom_cos_in;                      // cone: every ray whose angle to the axis has a larger cosine is imaged
+  double dom_cos_margin, dom_sin_margin;  // cos / sin of the dominance margin
+  int dominance;                          // 1: per-tile dominance cull of the frame list (needs the inner bounds above)
   const double* exact_data;               // device array [n_frames][8]: inverse(T_G_C) as the reference forms it —
                                           // conjugate quaternion (w, x, y, z), translation -(q^-1).rotate(t), pad
 };
@@ -253,6 +251,40 @@ __device__ __forceinline__ double observation_angle(double xc, double yc, double
   return asin(fabs(zc) / sqrt(xc * xc + yc * yc + zc * zc));
 }
 
+// Layer value of a texel (:194-206).  Colour: cv::Vec3b is (B,G,R) and grid_map::colorVectorToValue packs 0x00RRGGBB,
+// moved as raw bits (int(float(c/255.0)*255.0f) == c for every byte c; tests/test_oracle_ortho.py checks all 256).
+__device__ __forceinline__ float texel_value(const uint8_t* texel, int colored) {
+  if (colored) {
+    const unsigned int b = __ldg(texel), g = __ldg(texel + 1), r = __ldg(texel + 2);
+    return __uint_as_float((r << 16) | (g << 8) | b);
+  }
+  return static_cast<float>(__ldg(texel));
+}
+
+// Frame f (index within the launch) won `cell` with angle `angle` and keypoint (kx, ky): write the angle and the frame
+// index (:181-182; :183 num_observations += num_observations keeps 0 at 0, the layer is untouched), then the pixel is
+// round(keypoint), half away from zero, clamped to the last row / column (:186-193).  SELECT records the pixel and
+// grows the frame's bounding box in shared memory; otherwise the texel is fetched.  (The keypoint is taken by reference:
+// it may sit in local memory after the exact path, and is then read where the pixel is rounded, not at the call.)
+template <bool SELECT>
+__device__ __forceinline__ void store_winner(const OrthoArgs& a, int* s_bbox, size_t cell, int f, float angle,
+                                             const double& kx, const double& ky) {
+  a.elevation_angle[cell] = angle;
+  a.observation_index[cell] = static_cast<float>(a.frame_base + f);
+  const int py = min(static_cast<int>(round(ky)), a.height - 1);
+  const int px = min(static_cast<int>(round(kx)), a.width - 1);
+  if (SELECT) {
+    a.pix[cell] = (static_cast<unsigned int>(py) << 16) | static_cast<unsigned int>(px);
+    atomicMin(&s_bbox[f], px);
+    atomicMin(&s_bbox[kMaxFramesPerLaunch + f], py);
+    atomicMax(&s_bbox[2 * kMaxFramesPerLaunch + f], px);
+    atomicMax(&s_bbox[3 * kMaxFramesPerLaunch + f], py);
+  } else {
+    const uint8_t* texel = a.images[f] + static_cast<size_t>(py) * a.row_step + static_cast<size_t>(px) * a.channels;
+    a.out_layer[cell] = texel_value(texel, a.colored);
+  }
+}
+
 // One block = one OTI x OTJ cell tile; one thread = a 1 x kOStrip strip of cells (same i, adjacent j): the
 // per-frame constants are fetched once per thread and serve four cells, and the tile's cull list is built once
 // for 1024 cells.
@@ -260,16 +292,408 @@ __device__ __forceinline__ double observation_angle(double xc, double yc, double
 // SELECT = true:  phase A of the host-frame path: no texel access at all; records the winner's pixel per cell and
 //                 the bounding box of the winners' pixels per frame, so that only those sub-rectangles of the
 //                 host frames have to cross PCIe (phase B: ortho_texel_kernel).
-#define AMB_ORTHO_DOM 0
-#define AMB_ORTHO_KERNEL_NAME ortho_kernel
-#include "ortho_kernel_body.inc"
-#undef AMB_ORTHO_DOM
-#undef AMB_ORTHO_KERNEL_NAME
-#define AMB_ORTHO_DOM 1
-#define AMB_ORTHO_KERNEL_NAME ortho_kernel_dom
-#include "ortho_kernel_body.inc"
-#undef AMB_ORTHO_DOM
-#undef AMB_ORTHO_KERNEL_NAME
+//
+// The frame list is culled by conservative view cone / rectangle tests (unless a.do_cull == 0: brute force) and, with
+// a.dominance, by the per-tile DOMINANCE cull:
+//   alpha = asin(|z_c| / |X - c|) = pi/2 - theta, theta = angle between the ray and the optical axis.  Over the
+//   tile's bounding sphere (centre C, radius rho) theta lies in [max(0, theta_c - delta), theta_c + delta],
+//   theta_c = angle(axis, C - c), delta = asin(rho / |C - c|).  If a frame g sees EVERY landmark of the tile (sphere
+//   in front of the camera and inside the view rectangle shrunk by the distortion bound), any frame f with
+//   theta_min(f) > theta_max(g) + margin has a smaller alpha than g in every cell, by far more than the float32
+//   rounding of the running best can hide: whether or not f is visited, the reference's sequential recurrence ends
+//   in the same (angle, index) — after g has been visited the state is the same, and a frame between them that wins
+//   against the state without f also wins against the state with f or loses to g afterwards.  Dropping f therefore
+//   changes no output bit (tools/ortho_dominance_study.py checks this against the oracle) and leaves ~1.2 instead of
+//   ~8.5 frames per tile at the benchmark geometry.
+template <int DIST, bool SELECT>
+__global__ void __launch_bounds__(kOrthoThreads, AMB_OBPS) ortho_kernel_dom(const __grid_constant__ OrthoArgs a) {
+  __shared__ unsigned short s_list[kMaxFramesPerLaunch];
+  __shared__ int s_bbox[SELECT ? 4 * kMaxFramesPerLaunch : 4];
+  __shared__ float s_red[2][kOrthoThreads / 32];
+  __shared__ int s_warp_cnt[kOrthoThreads / 32];
+  __shared__ int s_total;
+
+  const int ti = threadIdx.x & 31, tq = threadIdx.x >> 5;
+  const int tiles_i = (a.rows + OTI - 1) / OTI;
+  const int i0 = (blockIdx.x % tiles_i) * OTI;
+  const int j0 = (blockIdx.x / tiles_i) * OTJ;
+  // ti / tq = lane / warp; a warp covers 32 consecutive rows of one strip column group (OTI may span several warps)
+  const int i = i0 + (tq % (OTI / 32)) * 32 + ti;
+  const int jl0 = j0 + kOStrip * (tq / (OTI / 32));
+
+  float elev[kOStrip];
+  unsigned int validmask = 0;
+  float zmin = FLT_MAX, zmax = -FLT_MAX;
+#pragma unroll
+  for (int m = 0; m < kOStrip; ++m) {
+    elev[m] = __int_as_float(0x7fc00000);
+    if (i < a.rows && jl0 + m < a.cols_slab) elev[m] = a.elevation[static_cast<size_t>(jl0 + m) * a.rows + i];
+    if (!isnan(elev[m])) {  // NaN elevation: every comparison is false, the cell stays untouched
+      validmask |= 1u << m;
+      zmin = fminf(zmin, elev[m]);
+      zmax = fmaxf(zmax, elev[m]);
+    }
+  }
+  // tile elevation range
+  for (int o = 16; o > 0; o >>= 1) {
+    zmin = fminf(zmin, __shfl_xor_sync(0xffffffffu, zmin, o));
+    zmax = fmaxf(zmax, __shfl_xor_sync(0xffffffffu, zmax, o));
+  }
+  if (ti == 0) {
+    s_red[0][tq] = zmin;
+    s_red[1][tq] = zmax;
+  }
+  if (threadIdx.x == 0) s_total = 0;
+  if (SELECT) {
+    for (int e = threadIdx.x; e < 2 * kMaxFramesPerLaunch; e += kOrthoThreads) {
+      s_bbox[e] = 0x7fffffff;                            // xmin, ymin
+      s_bbox[2 * kMaxFramesPerLaunch + e] = -1;          // xmax, ymax
+    }
+  }
+  __syncthreads();
+  zmin = s_red[0][0];
+  zmax = s_red[1][0];
+#pragma unroll
+  for (int w = 1; w < kOrthoThreads / 32; ++w) {
+    zmin = fminf(zmin, s_red[0][w]);
+    zmax = fmaxf(zmax, s_red[1][w]);
+  }
+  if (zmin > zmax) return;  // no cell of this tile has an elevation
+
+  // bounding sphere of the tile's landmarks (cell centres x elevation range)
+  const int i1 = min(i0 + OTI, a.rows) - 1, j1 = min(j0 + OTJ, a.cols_slab) - 1;
+  const double x_hi = a.base_x - a.res * i0, x_lo = a.base_x - a.res * i1;
+  const double y_hi = a.base_y - a.res * (a.col_begin + j0), y_lo = a.base_y - a.res * (a.col_begin + j1);
+  const double sx = 0.5 * (x_hi + x_lo), sy = 0.5 * (y_hi + y_lo);
+  const double sz = 0.5 * (static_cast<double>(zmin) + static_cast<double>(zmax));
+  const double ex = 0.5 * (x_hi - x_lo), ey = 0.5 * (y_hi - y_lo);
+  const double ez = 0.5 * (static_cast<double>(zmax) - static_cast<double>(zmin));
+  const double rho = sqrt(ex * ex + ey * ey + ez * ez) * (1.0 + 1e-9) + 1e-6;
+
+  {
+    // The angles are compared through their COSINES (cos is decreasing on [0, pi]), built from the sphere centre's camera
+    // coordinates with the addition formulas — no atan2 / asin per (tile, frame), which was 23 % of the kernel's
+    // instructions (the cull only has to be SOUND, not to reproduce a particular rounding: whichever frames it drops,
+    // the output is the same by the argument above):
+    //   cos(theta_c) = z_c / |C - c|, sin(theta_c) = perp / |C - c|, sin(delta) = rho / |C - c|
+    //   cos(theta_min) = 1 if theta_c <= delta, else cos(theta_c - delta);   cos(theta_max) = cos(theta_c + delta)
+    __shared__ double s_cmin[kMaxFramesPerLaunch];     // cos(theta_min) per surviving frame, NaN: not a candidate
+    __shared__ unsigned long long s_best_cmax;         // largest cos(theta_max) among the frames that see the whole tile
+    // pass 1: the conservative visibility tests, plus cos(theta_min) per surviving frame and (a.dominance) the largest
+    // cos(theta_max) among the frames that see the whole tile (doubles > 0 order like their bit patterns: atomicMax)
+    if (threadIdx.x == 0) s_best_cmax = 0ull;  // no whole-tile frame yet (theirs are > 0: the sphere is in front of them)
+    __syncthreads();
+    for (int f = threadIdx.x; f < a.n_frames; f += kOrthoThreads) {
+      // per-thread frame index: read from global memory (a divergent __constant__ index would serialise)
+      const double* cf = a.cull_data + 12 * static_cast<size_t>(f);
+      const double dx = sx - __ldg(cf + 0), dy = sy - __ldg(cf + 1), dz = sz - __ldg(cf + 2);
+      const double xp = dx * __ldg(cf + 3) + dy * __ldg(cf + 4) + dz * __ldg(cf + 5);    // x_c of the centre
+      const double yp = dx * __ldg(cf + 6) + dy * __ldg(cf + 7) + dz * __ldg(cf + 8);    // y_c
+      const double zp = dx * __ldg(cf + 9) + dy * __ldg(cf + 10) + dz * __ldg(cf + 11);  // z_c (optical axis)
+      const double dd = dx * dx + dy * dy + dz * dz;
+      const double slack = rho + 1e-9 * (fabs(xp) + fabs(yp) + fabs(zp));
+      const double perp = sqrt(fmax(dd - zp * zp, 0.0));
+      bool keep = true;
+      if (zp + rho <= 0.0) {
+        keep = false;  // whole sphere behind the camera plane: z_c <= 0 for every landmark
+      } else {
+        // distance from the sphere centre to the solid cone {angle to axis <= theta_c} is at least
+        // perp*cos(theta_c) - zp*sin(theta_c)
+        if (a.cone) {
+          if (perp * a.cos_c - zp * a.sin_c > slack) keep = false;
+        }
+        // a landmark with z_c > 0 and u = x_c/z_c > u_hi has x_c - u_hi*z_c > 0: the sphere lies entirely on
+        // that side of the plane through the camera centre iff the centre's value exceeds rho*|normal|
+        if (a.rect) {
+          if (xp - a.u_hi * zp > slack * a.nu_hi) keep = false;
+          if (a.u_lo * zp - xp > slack * a.nu_lo) keep = false;
+          if (yp - a.v_hi * zp > slack * a.nv_hi) keep = false;
+          if (a.v_lo * zp - yp > slack * a.nv_lo) keep = false;
+        }
+      }
+      double c_min = __longlong_as_double(0x7ff8000000000000ll);  // NaN: not a candidate
+      if (keep) {
+        const double inv = 1.0 / sqrt(dd);  // (dd == 0: inf — the camera sits on the sphere centre)
+        double c_max = -1.0;
+        c_min = 1.0;  // camera inside the tile's sphere: theta_min = 0 and the frame cannot "see the whole tile"
+        if (rho * inv < 1.0) {
+          const double cos_t = zp * inv, sin_t = perp * inv;
+          const double sin_d = rho * inv;
+          const double cos_d = sqrt(fmax(1.0 - sin_d * sin_d, 0.0));
+          c_min = cos_t >= cos_d ? 1.0 : cos_t * cos_d + sin_t * sin_d;
+          c_max = cos_t * cos_d - sin_t * sin_d;
+        }
+        // every landmark of the tile is imaged by this frame: pinhole / rad-tan — sphere inside the INNER view rectangle;
+        // equidistant / FOV — sphere inside the INNER view cone (every ray whose angle to the axis has a cosine above
+        // dom_cos_in lands in the raster; with the sphere in front of the camera theta_c + delta < pi/2, so the cosines
+        // compare like the angles)
+        const bool whole = a.dominance && zp - rho > 1e-6 && c_max > 0.0 &&
+                           (a.rect ? (xp - a.ui_hi * zp < -slack * a.nui_hi && a.ui_lo * zp - xp < -slack * a.nui_lo &&
+                                      yp - a.vi_hi * zp < -slack * a.nvi_hi && a.vi_lo * zp - yp < -slack * a.nvi_lo)
+                                   : (c_max > a.dom_cos_in + 1e-12));
+        if (whole) atomicMax(&s_best_cmax, static_cast<unsigned long long>(__double_as_longlong(c_max)));
+      }
+      s_cmin[f] = a.do_cull ? c_min : 1.0;  // brute force: every frame is a candidate (and a.dominance is 0)
+    }
+    __syncthreads();
+    // a frame is dropped when theta_min > theta_max(best) + margin, i.e. cos(theta_min) < cos(theta_max + margin)
+    // (1e-12 covers the rounding of the products above; the margin itself is 1e-4 rad)
+    double c_cut = -2.0;  // no whole-tile frame (always so without a.dominance): nothing is dropped
+    if (s_best_cmax != 0ull) {
+      const double c = __longlong_as_double(static_cast<long long>(s_best_cmax));
+      c_cut = c * a.dom_cos_margin - sqrt(fmax(1.0 - c * c, 0.0)) * a.dom_sin_margin - 1e-12;
+    }
+    // pass 2: ascending list of the candidates no whole-tile frame dominates
+    for (int f0 = 0; f0 < a.n_frames; f0 += kOrthoThreads) {
+      const int f = f0 + threadIdx.x;
+      bool keep = false;
+      if (f < a.n_frames) {
+        const double c_min = s_cmin[f];
+        keep = c_min == c_min && !(c_min < c_cut);
+      }
+      const unsigned int mk = __ballot_sync(0xffffffffu, keep);
+      if (ti == 0) s_warp_cnt[tq] = __popc(mk);
+      __syncthreads();
+      int before = s_total;
+      for (int w = 0; w < tq; ++w) before += s_warp_cnt[w];
+      if (keep) s_list[before + __popc(mk & ((1u << ti) - 1u))] = static_cast<unsigned short>(f);
+      __syncthreads();
+      if (threadIdx.x == 0) {
+        int t = s_total;
+        for (int w = 0; w < kOrthoThreads / 32; ++w) t += s_warp_cnt[w];
+        s_total = t;
+      }
+      __syncthreads();
+    }
+  }
+  const int n_list = s_total;
+#ifdef AMB_CUDA_EMU  // tests/emu only: how many frames the tile keeps (plain vs dominance cull)
+  if (threadIdx.x == 0) emu::note(a.dominance ? "ortho_dom_list" : "ortho_list", n_list);
+#endif
+  if (n_list == 0) return;
+  if (!SELECT && !validmask) return;  // (SELECT: every thread reaches the block-wide bbox flush below)
+
+  // ---- winner selection: the reference's recurrence  `alpha_f > (double)best_f32  =>  best_f32 = (float)alpha_f`
+  // with alpha = asin(|z|/norm)  (ortho-backward-grid.cc:173-183), evaluated WITHOUT an asin per candidate.
+  // asin is increasing with slope >= 1, so comparing s2 = z^2/norm^2 = sin^2(alpha) decides the comparison
+  // whenever the gap is larger than what the float32 rounding of the running best can hide:
+  //   running best known exactly (layer value b):          ref2 = sin^2(b), band 1e-11
+  //   running best = (float)asin(s_p) of a pending winner: ref2 = s_p^2,    band 2e-7
+  //       (|(float)a - a| <= 6.0e-8 * a <= 9.4e-8;  s2_f - s2_p > 2e-7  =>  s_f - s_p > 1e-7  =>  alpha_f - alpha_p > 1e-7)
+  // Inside the band the decision is made exactly as the reference does (asin of both, float-rounded best).
+  const double X = __dadd_rn(a.base_x, __dmul_rn(a.res, -static_cast<double>(i)));
+  double Y[kOStrip], Z[kOStrip], thr_hi[kOStrip], thr_lo[kOStrip];
+  float best[kOStrip];
+  int best_f[kOStrip];
+  unsigned int pending = 0;  // bit m: best_f[m] won but (float)asin(...) has not been evaluated yet
+#pragma unroll
+  for (int m = 0; m < kOStrip; ++m) {
+    Y[m] = __dadd_rn(a.base_y, __dmul_rn(a.res, -static_cast<double>(a.col_begin + jl0 + m)));
+    Z[m] = static_cast<double>(elev[m]);
+    best[m] = 0.0f;
+    best_f[m] = -1;
+    double ref2 = 4.0, band = 0.0;  // invalid cell: nothing can win
+    if ((validmask >> m) & 1u) {
+      best[m] = a.elevation_angle[static_cast<size_t>(jl0 + m) * a.rows + i];
+      if (best[m] > 0.0f) {
+        const double sb = sin(static_cast<double>(best[m]));
+        ref2 = sb * sb;
+        band = 1e-11;
+      } else if (best[m] == 0.0f) {
+        ref2 = 0.0;  // any visible frame has alpha > 0
+      } else if (best[m] < 0.0f) {
+        ref2 = -1.0;  // a negative layer value is beaten by anything; NaN (ref2 = 4) by nothing
+      }
+    }
+    thr_hi[m] = ref2 + band;
+    thr_lo[m] = ref2 - band;
+  }
+  bool check_failed = false;
+  unsigned int dirty = 0;  // bit m: a candidate fell inside a band (angle tie / raster edge / camera plane) -> redo exactly
+  const double wd = static_cast<double>(a.width), hd = static_cast<double>(a.height);
+
+  // ---- one candidate frame (after the dominance cull: ~4 of 5 tiles at the benchmark geometry) ----
+  // The frame loop below projects the winner a second time after its frame loop (like the reference, :186-188) because
+  // keeping every cell's winning keypoint across the loop costs registers; with a single candidate there is no loop state:
+  // each cell is evaluated, decided (exact re-evaluation included) and written in one go, from the SAME camera
+  // coordinates and keypoint (to_camera / project are the expressions of the loop body: identical bits).  The winner's
+  // re-projection was a third of the kernel's instructions.
+  if (n_list == 1) {  // block-uniform
+    const int f = s_list[0];
+    const FrameConst& fc = c_frames[f];
+    const double cx = fma(fc.m[0], X, fc.t[0]);
+    const double cy = fma(fc.m[3], X, fc.t[1]);
+    const double cz = fma(fc.m[6], X, fc.t[2]);
+#pragma unroll
+    for (int m = 0; m < kOStrip; ++m) {
+      if (!((validmask >> m) & 1u)) continue;   // no elevation / beyond the map edge: untouched, nothing is read
+      double xc = fma(fc.m[1], Y[m], fma(fc.m[2], Z[m], cx));
+      double yc = fma(fc.m[4], Y[m], fma(fc.m[5], Z[m], cy));
+      double zc = fma(fc.m[7], Y[m], fma(fc.m[8], Z[m], cz));
+      double kx, ky;
+      project<DIST>(a, xc, yc, zc, &kx, &ky);
+      const bool vis = kx >= kGuardPx && ky >= kGuardPx && kx < wd - kGuardPx && ky < hd - kGuardPx && zc > kGuardZ;
+      const bool out = kx < -kGuardPx || ky < -kGuardPx || kx >= wd + kGuardPx || ky >= hd + kGuardPx || zc < -kGuardZ;
+      const double z2 = zc * zc;
+      const double n2 = fma(xc, xc, fma(yc, yc, z2));
+      bool win = vis && (z2 > thr_hi[m] * n2);
+      const bool unc = (vis && !win && (z2 >= thr_lo[m] * n2)) || (!vis && !out);
+      bool pend = win;
+      float b = best[m];
+      if (unc) {  // too close to call: the reference's own operation sequence decides (as in the general path's dirty branch)
+        win = false;
+        pend = false;
+        double ex, ey, ez, ekx, eky;
+        exact_to_camera(a, f, X, Y[m], Z[m], &ex, &ey, &ez);
+        if (exact_project<DIST>(a, ex, ey, ez, &ekx, &eky)) {
+          const double alpha = exact_observation_angle(ex, ey, ez);
+          if (!(alpha > 0.0)) check_failed = true;  // reference: CHECK(alpha > 0.0), :178
+          if (alpha > static_cast<double>(b)) {     // :180
+            b = static_cast<float>(alpha);          // :181
+            win = true;
+          }
+        }
+      }
+      if (!win) continue;
+      const size_t cell = static_cast<size_t>(jl0 + m) * a.rows + i;
+      // the pixel is round(keypoint) (:186-193): within the guard of a half-integer (or for a cell that took the exact
+      // path) the keypoint is recomputed with the reference's operation sequence
+      const bool near_half = fabs((kx - floor(kx)) - 0.5) < kGuardPx || fabs((ky - floor(ky)) - 0.5) < kGuardPx;
+      if (near_half || unc || !(kx == kx) || !(ky == ky)) {
+        exact_to_camera(a, f, X, Y[m], Z[m], &xc, &yc, &zc);
+        exact_project<DIST>(a, xc, yc, zc, &kx, &ky);
+      }
+      if (pend) {
+        const double alpha = observation_angle(xc, yc, zc);
+        if (!(alpha > 0.0)) check_failed = true;
+        b = static_cast<float>(alpha);
+      }
+      store_winner<SELECT>(a, s_bbox, cell, f, b, kx, ky);
+    }
+    // Own exit rather than a fall-through into the shared flush below: joining the two paths keeps n_list and the flag
+    // live across this block, and ptxas then spills more in three of the SELECT instances and reschedules this block.
+    if (check_failed) atomicExch(a.error_flag, 1u);
+    if (SELECT) {
+      __syncthreads();
+      if (threadIdx.x == 0 && s_bbox[2 * kMaxFramesPerLaunch + f] >= 0) {
+        int* g = a.bbox + 4 * (a.frame_base + f);
+        atomicMin(g + 0, s_bbox[f]);
+        atomicMin(g + 1, s_bbox[kMaxFramesPerLaunch + f]);
+        atomicMax(g + 2, s_bbox[2 * kMaxFramesPerLaunch + f]);
+        atomicMax(g + 3, s_bbox[3 * kMaxFramesPerLaunch + f]);
+      }
+    }
+    return;
+  }
+
+  // Hot loop: straight-line code, four independent dependency chains per thread (one per cell of the strip).
+  for (int l = 0; l < n_list; ++l) {
+    const int f = s_list[l];
+    const FrameConst& fc = c_frames[f];
+    const double cx = fma(fc.m[0], X, fc.t[0]);
+    const double cy = fma(fc.m[3], X, fc.t[1]);
+    const double cz = fma(fc.m[6], X, fc.t[2]);
+#pragma unroll
+    for (int m = 0; m < kOStrip; ++m) {
+      const double xc = fma(fc.m[1], Y[m], fma(fc.m[2], Z[m], cx));
+      const double yc = fma(fc.m[4], Y[m], fma(fc.m[5], Z[m], cy));
+      const double zc = fma(fc.m[7], Y[m], fma(fc.m[8], Z[m], cz));
+      double kx, ky;
+      project<DIST>(a, xc, yc, zc, &kx, &ky);
+      // visibility with a guard band (kGuardPx / kGuardZ): certainly inside, certainly not visible, or too close to call
+      // with FMA-contracted coordinates (NaN keypoints compare false everywhere: too close to call) -> exact path
+      const bool vis = kx >= kGuardPx && ky >= kGuardPx && kx < wd - kGuardPx && ky < hd - kGuardPx && zc > kGuardZ;
+      const bool out = kx < -kGuardPx || ky < -kGuardPx || kx >= wd + kGuardPx || ky >= hd + kGuardPx || zc < -kGuardZ;
+      const double z2 = zc * zc;
+      const double n2 = fma(xc, xc, fma(yc, yc, z2));
+      const bool win = vis && (z2 > thr_hi[m] * n2);
+      // (cells without an elevation — NaN, or beyond the map edge in a partial tile — have NaN keypoints: never "too
+      // close to call", nothing can win there and their layer entries must not even be read)
+      const bool unc = (vis && !win && (z2 >= thr_lo[m] * n2)) || (!vis && !out && ((validmask >> m) & 1u));
+      dirty |= (unc ? 1u : 0u) << m;
+      const double ref2 = z2 * fast_rcp(n2);
+      best_f[m] = win ? f : best_f[m];
+      thr_hi[m] = win ? ref2 + 2e-7 : thr_hi[m];
+      thr_lo[m] = win ? ref2 - 2e-7 : thr_lo[m];
+      pending |= (win ? 1u : 0u) << m;
+    }
+  }
+
+  if (dirty) {
+    // Rare (a near-tie within the float32 rounding of the running best, a keypoint within 1e-9 px of the raster edge, a
+    // landmark on the camera plane): evaluate the reference's recurrence literally for those cells, with the
+    // reference's own operation sequence (exact_*: quaternion rotation, IEEE division, no contraction) — asin for
+    // every visible frame, float-rounded best (:173-183).
+#pragma unroll
+    for (int m = 0; m < kOStrip; ++m) {  // unrolled: the per-cell arrays must stay in registers
+      if (!((dirty >> m) & 1u)) continue;
+      float b = a.elevation_angle[static_cast<size_t>(jl0 + m) * a.rows + i];
+      int bf = -1;
+      for (int l = 0; l < n_list; ++l) {
+        const int f = s_list[l];
+        double xc, yc, zc, kx, ky;
+        exact_to_camera(a, f, X, Y[m], Z[m], &xc, &yc, &zc);
+        if (!exact_project<DIST>(a, xc, yc, zc, &kx, &ky)) continue;
+        const double alpha = exact_observation_angle(xc, yc, zc);
+        if (!(alpha > 0.0)) check_failed = true;  // reference: CHECK(alpha > 0.0), :178
+        if (alpha > static_cast<double>(b)) {     // :180
+          b = static_cast<float>(alpha);          // :181
+          bf = f;
+        }
+      }
+      best[m] = b;
+      best_f[m] = bf;
+      pending &= ~(1u << m);
+    }
+  }
+
+#pragma unroll
+  for (int m = 0; m < kOStrip; ++m) {
+    if (best_f[m] < 0) continue;
+    const size_t cell = static_cast<size_t>(jl0 + m) * a.rows + i;
+    // the winner's camera coordinates and keypoint, recomputed (the reference projects a second time too, :186-188)
+    double xc, yc, zc, kx, ky;
+    to_camera(best_f[m], X, Y[m], Z[m], &xc, &yc, &zc);
+    project<DIST>(a, xc, yc, zc, &kx, &ky);
+    // the pixel is round(keypoint) (:186-193): within the guard of a half-integer (or for a cell that already took the
+    // exact path) the keypoint is recomputed with the reference's operation sequence
+    const bool near_half = fabs((kx - floor(kx)) - 0.5) < kGuardPx || fabs((ky - floor(ky)) - 0.5) < kGuardPx;
+    if (near_half || ((dirty >> m) & 1u) || !(kx == kx) || !(ky == ky)) {
+      exact_to_camera(a, best_f[m], X, Y[m], Z[m], &xc, &yc, &zc);
+      exact_project<DIST>(a, xc, yc, zc, &kx, &ky);
+    }
+    if ((pending >> m) & 1u) {
+      const double alpha = observation_angle(xc, yc, zc);
+      if (!(alpha > 0.0)) check_failed = true;
+      best[m] = static_cast<float>(alpha);
+    }
+    store_winner<SELECT>(a, s_bbox, cell, best_f[m], best[m], kx, ky);
+  }
+  if (check_failed) atomicExch(a.error_flag, 1u);
+  if (SELECT) {
+    __syncthreads();
+    for (int l = threadIdx.x; l < n_list; l += kOrthoThreads) {
+      const int f = s_list[l];
+      if (s_bbox[2 * kMaxFramesPerLaunch + f] >= 0) {
+        int* g = a.bbox + 4 * (a.frame_base + f);
+        atomicMin(g + 0, s_bbox[f]);
+        atomicMin(g + 1, s_bbox[kMaxFramesPerLaunch + f]);
+        atomicMax(g + 2, s_bbox[2 * kMaxFramesPerLaunch + f]);
+        atomicMax(g + 3, s_bbox[3 * kMaxFramesPerLaunch + f]);
+      }
+    }
+  }
+}
+
+template <bool SELECT>
+void launch_ortho_kernel(const OrthoArgs& a, int grid, cudaStream_t s) {
+  switch (a.dist_type) {
+    case AMB_DIST_RADTAN: ortho_kernel_dom<AMB_DIST_RADTAN, SELECT><<<grid, kOrthoThreads, 0, s>>>(a); break;
+    case AMB_DIST_EQUIDISTANT: ortho_kernel_dom<AMB_DIST_EQUIDISTANT, SELECT><<<grid, kOrthoThreads, 0, s>>>(a); break;
+    case AMB_DIST_FOV: ortho_kernel_dom<AMB_DIST_FOV, SELECT><<<grid, kOrthoThreads, 0, s>>>(a); break;
+    default: ortho_kernel_dom<AMB_DIST_NONE, SELECT><<<grid, kOrthoThreads, 0, s>>>(a);
+  }
+}
 
 // Bounding boxes device -> HOST-MAPPED pinned memory with plain stores: the read-back must not queue behind the
 // result layers that are streaming to the host on the device->host copy engine.
@@ -298,12 +722,7 @@ __global__ void __launch_bounds__(256) ortho_texel_kernel(const unsigned int* __
     const FrameRect r = rects[f];
     const int px = static_cast<int>(p & 0xffffu), py = static_cast<int>(p >> 16);
     const uint8_t* texel = r.ptr + static_cast<size_t>(py - r.y0) * r.pitch + static_cast<size_t>(px - r.x0) * channels;
-    if (colored) {
-      const unsigned int b = __ldg(texel), g = __ldg(texel + 1), rr = __ldg(texel + 2);
-      out_layer[cell] = __uint_as_float((rr << 16) | (g << 8) | b);
-    } else {
-      out_layer[cell] = static_cast<float>(__ldg(texel));
-    }
+    out_layer[cell] = texel_value(texel, colored);
   }
 }
 
@@ -591,70 +1010,60 @@ int ortho_run(amb_ctx* ctx, const amb_camera* camera, const double* T_G_B, const
     a.nv_hi = std::sqrt(1.0 + a.v_hi * a.v_hi);
   }
 
-  // Dominance cull (opt-in, amb_ortho_set_dominance_cull): needs the view rectangle (pinhole / rad-tan) and a
-  // non-empty INNER rectangle — the raster's normalised extent shrunk by the same distortion bound E the outer
-  // rectangle was grown by: a ray with an undistorted keypoint inside it is imaged inside the raster.
-  bool dominance = false;
-  if (ctx->ortho_dominance && a.do_cull && a.cone && !a.rect && a.dist_type == AMB_DIST_EQUIDISTANT) {
-    // Equidistant: the keypoint's distance from the principal point (normalised) is |theta * poly(theta^2)| whatever the
-    // azimuth, so every ray with theta <= theta_in is imaged if that radius stays below the distance to the nearest
-    // raster edge on [0, theta_in].  Scan outwards with a Lipschitz bound on the radius; stop at the first step that
-    // might leave the inscribed circle.
-    const double* k = camera->dist;
-    const double r_in = std::min(std::min(camera->cu, camera->width - camera->cu) / std::fabs(camera->fu),
-                                 std::min(camera->cv, camera->height - camera->cv) / std::fabs(camera->fv)) * (1.0 - 1e-9);
-    const double step = 1e-4;
-    double th = 0.0;
-    while (th < 1.5) {
-      const double b = th + step, b2 = b * b;
-      const double lip = 1.0 + 3.0 * std::fabs(k[0]) * b2 + 5.0 * std::fabs(k[1]) * b2 * b2 +
-                         7.0 * std::fabs(k[2]) * b2 * b2 * b2 + 9.0 * std::fabs(k[3]) * b2 * b2 * b2 * b2;  // >= |d r / d theta|
-      const double t2 = th * th;
-      const double r_th = std::fabs(th * (1.0 + k[0] * t2 + k[1] * t2 * t2 + k[2] * t2 * t2 * t2 + k[3] * t2 * t2 * t2 * t2));
-      if (r_th + lip * step >= r_in) break;
-      th = b;
-    }
-    if (th > 1e-3 && camera->fu > 0.0 && camera->fv > 0.0) {
-      a.dom_theta_in = th;
-      a.dom_margin = 1e-4;
-      dominance = true;
-    }
-  } else if (ctx->ortho_dominance && a.do_cull && a.cone && !a.rect && a.dist_type == AMB_DIST_FOV) {
-    // FOV: radius atan(2 tan(w/2) tan(theta)) / w, increasing — every ray with that radius below the distance to the
-    // nearest raster edge is imaged: tan(theta_in) = tan(w r_in) / (2 tan(w/2))
-    const double w = std::fabs(camera->dist[0]);
-    const double r_in = std::min(std::min(camera->cu, camera->width - camera->cu) / std::fabs(camera->fu),
-                                 std::min(camera->cv, camera->height - camera->cv) / std::fabs(camera->fv)) * (1.0 - 1e-9);
-    double tan_in = r_in;
-    if (w * w >= 1e-5) tan_in = (w * r_in < 1.5) ? std::tan(w * r_in) / (2.0 * std::fabs(std::tan(w / 2.))) : -1.0;
-    const double th = tan_in > 0.0 ? std::atan(tan_in) * (1.0 - 1e-9) : 0.0;
-    if (th > 1e-3 && camera->fu > 0.0 && camera->fv > 0.0) {
-      a.dom_theta_in = th;
-      a.dom_margin = 1e-4;
-      dominance = true;
-    }
-  } else if (ctx->ortho_dominance && a.do_cull && a.rect && a.dist_type != AMB_DIST_EQUIDISTANT) {
-    const double E_u = a.u_hi - (camera->width - camera->cu) / camera->fu;   // what compute_view_rect added
-    const double E_v = a.v_hi - (camera->height - camera->cv) / camera->fv;
-    const double E = std::max(E_u, E_v) * (1.0 + 1e-9) + 1e-9;
-    a.ui_lo = -camera->cu / camera->fu + E;
-    a.ui_hi = (camera->width - camera->cu) / camera->fu - E;
-    a.vi_lo = -camera->cv / camera->fv + E;
-    a.vi_hi = (camera->height - camera->cv) / camera->fv - E;
-    if (a.ui_lo < a.ui_hi && a.vi_lo < a.vi_hi) {
+  // Dominance cull (amb_ortho_set_dominance_cull): needs an INNER bound, a set of rays that are certainly imaged inside
+  // the raster.  r_in: normalised distance from the principal point to the nearest raster edge.
+  if (ctx->ortho_dominance && a.do_cull && a.cone && camera->fu > 0.0 && camera->fv > 0.0) {
+    const double r_in = std::min(std::min(camera->cu, camera->width - camera->cu) / camera->fu,
+                                 std::min(camera->cv, camera->height - camera->cv) / camera->fv) * (1.0 - 1e-9);
+    bool inner = false;
+    double th = 0.0;  // inner view cone (equidistant, FOV): every ray with angle-to-axis below th is imaged
+    if (a.rect) {
+      // Pinhole / rad-tan: the INNER rectangle, the raster's normalised extent shrunk by the same distortion bound E the
+      // outer rectangle was grown by: a ray with an undistorted keypoint inside it is imaged inside the raster.
+      const double E_u = a.u_hi - (camera->width - camera->cu) / camera->fu;   // what compute_view_rect added
+      const double E_v = a.v_hi - (camera->height - camera->cv) / camera->fv;
+      const double E = std::max(E_u, E_v) * (1.0 + 1e-9) + 1e-9;
+      a.ui_lo = -camera->cu / camera->fu + E;
+      a.ui_hi = (camera->width - camera->cu) / camera->fu - E;
+      a.vi_lo = -camera->cv / camera->fv + E;
+      a.vi_hi = (camera->height - camera->cv) / camera->fv - E;
       a.nui_lo = std::sqrt(1.0 + a.ui_lo * a.ui_lo);
       a.nui_hi = std::sqrt(1.0 + a.ui_hi * a.ui_hi);
       a.nvi_lo = std::sqrt(1.0 + a.vi_lo * a.vi_lo);
       a.nvi_hi = std::sqrt(1.0 + a.vi_hi * a.vi_hi);
-      a.dom_margin = 1e-4;  // rad; the float32 rounding of an angle <= pi/2 is < 1.2e-7
-      dominance = true;
+      inner = a.ui_lo < a.ui_hi && a.vi_lo < a.vi_hi;
+    } else if (a.dist_type == AMB_DIST_EQUIDISTANT) {
+      // Equidistant: the keypoint's distance from the principal point (normalised) is |theta * poly(theta^2)| whatever
+      // the azimuth, so every ray with theta <= th is imaged if that radius stays below r_in on [0, th].  Scan outwards
+      // with a Lipschitz bound on the radius; stop at the first step that might leave the inscribed circle.
+      const double* k = camera->dist;
+      const double step = 1e-4;
+      while (th < 1.5) {
+        const double b = th + step, b2 = b * b;
+        const double lip = 1.0 + 3.0 * std::fabs(k[0]) * b2 + 5.0 * std::fabs(k[1]) * b2 * b2 +
+                           7.0 * std::fabs(k[2]) * b2 * b2 * b2 + 9.0 * std::fabs(k[3]) * b2 * b2 * b2 * b2;  // >= |dr/dtheta|
+        const double t2 = th * th;
+        const double r_th = std::fabs(th * (1.0 + k[0] * t2 + k[1] * t2 * t2 + k[2] * t2 * t2 * t2 + k[3] * t2 * t2 * t2 * t2));
+        if (r_th + lip * step >= r_in) break;
+        th = b;
+      }
+      inner = th > 1e-3;
+    } else if (a.dist_type == AMB_DIST_FOV) {
+      // FOV: radius atan(2 tan(w/2) tan(theta)) / w, increasing — every ray with that radius below r_in is imaged:
+      // tan(th) = tan(w r_in) / (2 tan(w/2))
+      const double w = std::fabs(camera->dist[0]);
+      double tan_in = r_in;
+      if (w * w >= 1e-5) tan_in = (w * r_in < 1.5) ? std::tan(w * r_in) / (2.0 * std::fabs(std::tan(w / 2.))) : -1.0;
+      th = tan_in > 0.0 ? std::atan(tan_in) * (1.0 - 1e-9) : 0.0;
+      inner = th > 1e-3;
     }
-  }
-
-  if (dominance) {
-    a.dom_cos_in = std::cos(a.dom_theta_in);
-    a.dom_cos_margin = std::cos(a.dom_margin);
-    a.dom_sin_margin = std::sin(a.dom_margin);
+    if (inner) {
+      const double margin = 1e-4;  // rad; the float32 rounding of an angle <= pi/2 is < 1.2e-7
+      a.dominance = 1;
+      a.dom_cos_in = std::cos(th);
+      a.dom_cos_margin = std::cos(margin);
+      a.dom_sin_margin = std::sin(margin);
+    }
   }
   const int tiles_i = (a.rows + OTI - 1) / OTI, tiles_j = (a.cols_slab + OTJ - 1) / OTJ;
   ctx->ortho_launches = 0;
@@ -671,45 +1080,10 @@ int ortho_run(amb_ctx* ctx, const amb_camera* camera, const double* T_G_B, const
     a.images = ctx->frame_table.as<const uint8_t*>() + f0;
     a.cull_data = ctx->frame_cull.as<double>() + 12 * f0;
     a.exact_data = ctx->frame_cull.as<double>() + 12 * n + 8 * f0;
-    const int grid = tiles_i * tiles_j;
-    if (dominance) {
-      if (select_only) {
-        if (a.dist_type == AMB_DIST_RADTAN) {
-          ortho_kernel_dom<AMB_DIST_RADTAN, true><<<grid, kOrthoThreads, 0, s>>>(a);
-        } else if (a.dist_type == AMB_DIST_EQUIDISTANT) {
-          ortho_kernel_dom<AMB_DIST_EQUIDISTANT, true><<<grid, kOrthoThreads, 0, s>>>(a);
-        } else if (a.dist_type == AMB_DIST_FOV) {
-          ortho_kernel_dom<AMB_DIST_FOV, true><<<grid, kOrthoThreads, 0, s>>>(a);
-        } else {
-          ortho_kernel_dom<AMB_DIST_NONE, true><<<grid, kOrthoThreads, 0, s>>>(a);
-        }
-      } else if (a.dist_type == AMB_DIST_RADTAN) {
-        ortho_kernel_dom<AMB_DIST_RADTAN, false><<<grid, kOrthoThreads, 0, s>>>(a);
-      } else if (a.dist_type == AMB_DIST_EQUIDISTANT) {
-        ortho_kernel_dom<AMB_DIST_EQUIDISTANT, false><<<grid, kOrthoThreads, 0, s>>>(a);
-      } else if (a.dist_type == AMB_DIST_FOV) {
-        ortho_kernel_dom<AMB_DIST_FOV, false><<<grid, kOrthoThreads, 0, s>>>(a);
-      } else {
-        ortho_kernel_dom<AMB_DIST_NONE, false><<<grid, kOrthoThreads, 0, s>>>(a);
-      }
-    } else if (select_only) {
-      if (a.dist_type == AMB_DIST_RADTAN) {
-        ortho_kernel<AMB_DIST_RADTAN, true><<<grid, kOrthoThreads, 0, s>>>(a);
-      } else if (a.dist_type == AMB_DIST_EQUIDISTANT) {
-        ortho_kernel<AMB_DIST_EQUIDISTANT, true><<<grid, kOrthoThreads, 0, s>>>(a);
-      } else if (a.dist_type == AMB_DIST_FOV) {
-        ortho_kernel<AMB_DIST_FOV, true><<<grid, kOrthoThreads, 0, s>>>(a);
-      } else {
-        ortho_kernel<AMB_DIST_NONE, true><<<grid, kOrthoThreads, 0, s>>>(a);
-      }
-    } else if (a.dist_type == AMB_DIST_RADTAN) {
-      ortho_kernel<AMB_DIST_RADTAN, false><<<grid, kOrthoThreads, 0, s>>>(a);
-    } else if (a.dist_type == AMB_DIST_EQUIDISTANT) {
-      ortho_kernel<AMB_DIST_EQUIDISTANT, false><<<grid, kOrthoThreads, 0, s>>>(a);
-    } else if (a.dist_type == AMB_DIST_FOV) {
-      ortho_kernel<AMB_DIST_FOV, false><<<grid, kOrthoThreads, 0, s>>>(a);
+    if (select_only) {
+      launch_ortho_kernel<true>(a, tiles_i * tiles_j, s);
     } else {
-      ortho_kernel<AMB_DIST_NONE, false><<<grid, kOrthoThreads, 0, s>>>(a);
+      launch_ortho_kernel<false>(a, tiles_i * tiles_j, s);
     }
     ctx->ortho_launches += 1;
     AMB_CUDA(ctx, cudaEventRecord(guard_event, s));

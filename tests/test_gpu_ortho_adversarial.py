@@ -1,5 +1,5 @@
 """Orthomosaic decisions that sit EXACTLY on (or within rounding of) their boundaries — the cases the fused fast path of
-ortho_kernel cannot decide with FMA-contracted arithmetic and hands to the exact re-evaluation (csrc/ortho_kernels.cu:
+ortho_kernel_dom cannot decide with FMA-contracted arithmetic and hands to the exact re-evaluation (csrc/ortho_kernels.cu:
 kGuardPx / kGuardZ, exact_to_camera / exact_project).  Every scenario is compared with the CPU oracle and, when
 oracle/_ref is built, with the reference's own ortho-backward-grid.cc: observation_index and pixels must be identical.
 

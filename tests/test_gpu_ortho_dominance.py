@@ -1,5 +1,6 @@
-"""The per-tile DOMINANCE cull of the orthomosaic's frame list (ortho_kernel_dom, amb_ortho_set_dominance_cull;
-csrc/ortho_kernel_body.inc, DESIGN.md §4; the default since round 2): it must not change a single output bit.  Every
+"""The per-tile DOMINANCE cull of the orthomosaic's frame list (amb_ortho_set_dominance_cull; csrc/ortho_kernels.cu,
+DESIGN.md §4; the default since round 2): it must not change a single output bit.  Both cull modes run through the one
+kernel ortho_kernel_dom, the plain list with the dominance switch off.  Every
 scenario runs with the cull on and is compared (i) bit for bit with the same run without it (AMB_ORTHO_DOMINANCE=0) and
 (ii) with the CPU oracle.  The argument and the expected saving
 are also checked on the CPU by tools/ortho_dominance_study.py (oracle restricted to the surviving frames == full
