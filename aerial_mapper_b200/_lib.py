@@ -102,6 +102,11 @@ SYMBOLS = {
     "amb_dsm_thresholds": (C.c_int, [C.c_int32, _P, C.c_int32]),
     "amb_ortho_from_pcl_process": (C.c_int, [_P, _P, _P, C.c_size_t, C.c_int32, C.c_int32]),
     "amb_ortho_from_pcl_process_device": (C.c_int, [_P, _P, _P, C.c_size_t, C.c_int32, C.c_int32]),
+    "amb_ortho_from_pcl_process_device_ids": (C.c_int, [_P, _P, _P, _P, C.c_size_t, C.c_int32, C.c_int32]),
+    "amb_ortho_from_pcl_extract_halo": (C.c_int, [_P, _P, _P, _P, C.c_size_t, C.c_double, C.c_double, C.c_double, _P,
+                                                  _P, _P, C.c_uint32, _P]),
+    "amb_ortho_from_pcl_process_sharded_device": (C.c_int, [_P, _P, _P, _P, C.c_size_t, C.c_int32, C.c_uint32]),
+    "amb_ortho_from_pcl_process_sharded": (C.c_int, [_P, _P, _P, _P, C.c_size_t, C.c_int32, C.c_uint32]),
     "amb_stereo_reproject": (C.c_int, [C.c_int, _P, C.c_size_t, _P, C.c_size_t, C.c_int32, C.c_int32, _P, C.c_double,
                                        _P, _P, C.c_float, _P, _P, C.c_size_t, C.POINTER(C.c_size_t)]),
     "amb_stereo_reproject_device": (C.c_int, [C.c_int, _P, _P, C.c_size_t, _P, C.c_size_t, C.c_int32, C.c_int32, _P,
@@ -127,6 +132,7 @@ SYMBOLS = {
     "amb_multi_sync": (C.c_int, [_P]),
     "amb_multi_dsm_process": (C.c_int, [_P, _P, C.c_size_t, C.c_int32, C.c_double, C.c_double]),
     "amb_multi_ortho_process": (C.c_int, [_P, C.POINTER(Camera), _P, _P, C.c_size_t, C.c_int32, C.c_size_t, C.c_int32]),
+    "amb_multi_ortho_from_pcl_process": (C.c_int, [_P, _P, _P, C.c_size_t, C.c_int32, C.c_int32]),
     "amb_get_timings": (C.c_int, [_P, C.POINTER(Timings)]),
     "amb_host_alloc": (C.c_int, [C.POINTER(_P), C.c_size_t]),
     "amb_host_free": (C.c_int, [_P]),

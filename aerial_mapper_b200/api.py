@@ -491,6 +491,55 @@ class OrthoFromPcl(object):
         if not map.is_resident():
             map.download(("ortho",))
 
+    def process_device(self, d_xyz, d_intensities, n, map, d_ids=None):
+        """Points (float64 [n, 3]) and intensities (int32 [n]) already in HBM (device pointers as ints); asynchronous —
+        map.sync() before reading results.  d_ids: optional device pointer to one uint64 global id per point (a sharded
+        cloud), the canonical summation order instead of the array position."""
+        if n == 0:
+            raise AmbError(_lib.AMB_ERR_EMPTY, "CHECK(!pointcloud.empty()) (ortho-from-pcl.cc:23)")
+        ctx = map.context()
+        s = self.settings_
+        adaptive = 1 if s.use_adaptive_interpolation else 0
+        if d_ids is None:
+            check(lib().amb_ortho_from_pcl_process_device(ctx, C.c_void_p(int(d_xyz)), C.c_void_p(int(d_intensities)),
+                                                          int(n), int(s.interpolation_radius), adaptive), ctx)
+        else:
+            check(lib().amb_ortho_from_pcl_process_device_ids(ctx, C.c_void_p(int(d_xyz)),
+                                                              C.c_void_p(int(d_intensities)), C.c_void_p(int(d_ids)),
+                                                              int(n), int(s.interpolation_radius), adaptive), ctx)
+
+    def _no_adaptive_when_sharded(self):
+        if self.settings_.use_adaptive_interpolation:
+            raise AmbError(_lib.AMB_ERR_UNSUPPORTED,
+                           "adaptive interpolation needs the whole cloud, which no rank of a sharded cloud holds")
+
+    def process_sharded_device(self, d_xyz, d_intensities, d_ids, n_local, map, halo_capacity):
+        """A cloud sharded by stripe, the exchange step included (amb_ortho_from_pcl_process_sharded_device): this
+        rank's points, intensities and global ids (device pointers) -> the stripe's `ortho`.  Collective over the
+        communicator the map's context joined (sharding.init_comm); asynchronous — map.sync() before reading results."""
+        self._no_adaptive_when_sharded()
+        ctx = map.context()
+        check(lib().amb_ortho_from_pcl_process_sharded_device(ctx, C.c_void_p(int(d_xyz)), C.c_void_p(int(d_intensities)),
+                                                              C.c_void_p(int(d_ids)), int(n_local),
+                                                              int(self.settings_.interpolation_radius),
+                                                              int(halo_capacity)), ctx)
+
+    def process_sharded(self, pointcloud, intensities, ids, map, halo_capacity):
+        """Same with this rank's points (float64 [n, 3]), intensities (int32 [n]) and global ids (uint64 [n]) in host
+        memory."""
+        self._no_adaptive_when_sharded()
+        pc = np.ascontiguousarray(pointcloud, dtype=np.float64)
+        n = pc.size // 3
+        inten = np.ascontiguousarray(intensities, dtype=np.int32)
+        idv = np.ascontiguousarray(ids, dtype=np.uint64)
+        if inten.size < n or idv.size < n:
+            raise AmbError(_lib.AMB_ERR_SIZE_MISMATCH, "one intensity and one id per point")
+        ctx = map.context()
+        check(lib().amb_ortho_from_pcl_process_sharded(ctx, pc.ctypes.data_as(C.c_void_p),
+                                                       inten.ctypes.data_as(C.c_void_p), idv.ctypes.data_as(C.c_void_p),
+                                                       n, int(self.settings_.interpolation_radius),
+                                                       int(halo_capacity)), ctx)
+
 
 K_MAX_INVALID_DISPARITY = 1  # stereo::Densifier::kMaxInvalidDisparity (densifier.h:49)
 

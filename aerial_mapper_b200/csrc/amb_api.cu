@@ -373,8 +373,10 @@ int amb_dsm_process_device_ids(amb_ctx* ctx, const double* d_xyz, const uint64_t
 }
 
 // ---- OrthoFromPcl ("next" row N1, SURVEY.md §8f) ----
-int amb_ortho_from_pcl_process_device(amb_ctx* ctx, const double* d_xyz, const int32_t* d_intensities, size_t n,
-                                      int32_t interpolation_radius, int32_t use_adaptive_interpolation) {
+// d_ids: nullptr (array positions are the canonical order) or the caller's global point ids
+static int ortho_from_pcl_device(amb_ctx* ctx, const double* d_xyz, const int32_t* d_intensities,
+                                 const unsigned long long* d_ids, size_t n, int32_t interpolation_radius,
+                                 int32_t use_adaptive_interpolation) {
   if (!ctx) return AMB_ERR_INVALID_ARGUMENT;
   if (n == 0) return AMB_ERR_EMPTY;  // CHECK(!pointcloud.empty()), ortho-from-pcl.cc:23
   if (!d_xyz || !d_intensities) return AMB_ERR_INVALID_ARGUMENT;
@@ -385,12 +387,39 @@ int amb_ortho_from_pcl_process_device(amb_ctx* ctx, const double* d_xyz, const i
   float* saved = nullptr;  // adaptive interpolation (ortho-from-pcl.cc:63-72): pcl_adaptive_kernels.cu
   if (use_adaptive_interpolation) {
     const int pst = pcl_adaptive_prepare(ctx, &saved);
-    if (pst != AMB_OK) return pcl_adaptive_finish(ctx, pst, n, interpolation_radius, saved);
+    if (pst != AMB_OK)
+      return pcl_adaptive_finish(ctx, pst, d_xyz, d_ids, d_intensities, n, interpolation_radius, saved);
   }
-  int st = dsm_run(ctx, d_xyz, nullptr, n, interpolation_radius, 0.0, 0.0, 1, d_intensities);
-  if (use_adaptive_interpolation) st = pcl_adaptive_finish(ctx, st, n, interpolation_radius, saved);
+  int st = dsm_run(ctx, d_xyz, d_ids, n, interpolation_radius, 0.0, 0.0, 1, d_intensities);
+  if (use_adaptive_interpolation)
+    st = pcl_adaptive_finish(ctx, st, d_xyz, d_ids, d_intensities, n, interpolation_radius, saved);
   ctx->dsm_timed = (st == AMB_OK);
   return st;
+}
+
+int amb_ortho_from_pcl_process_device(amb_ctx* ctx, const double* d_xyz, const int32_t* d_intensities, size_t n,
+                                      int32_t interpolation_radius, int32_t use_adaptive_interpolation) {
+  return ortho_from_pcl_device(ctx, d_xyz, d_intensities, nullptr, n, interpolation_radius, use_adaptive_interpolation);
+}
+
+int amb_ortho_from_pcl_process_device_ids(amb_ctx* ctx, const double* d_xyz, const int32_t* d_intensities,
+                                          const uint64_t* d_ids, size_t n, int32_t interpolation_radius,
+                                          int32_t use_adaptive_interpolation) {
+  if (!d_ids) return AMB_ERR_INVALID_ARGUMENT;
+  return ortho_from_pcl_device(ctx, d_xyz, d_intensities, reinterpret_cast<const unsigned long long*>(d_ids), n,
+                               interpolation_radius, use_adaptive_interpolation);
+}
+
+int amb_ortho_from_pcl_extract_halo(amb_ctx* ctx, const double* d_xyz, const int32_t* d_intensities,
+                                    const uint64_t* d_ids, size_t n, double y_lo, double y_hi, double reach,
+                                    double* d_out_xyz, int32_t* d_out_intensities, uint64_t* d_out_ids,
+                                    uint32_t capacity, uint32_t* d_count) {
+  if (!ctx || !d_xyz || !d_intensities || !d_out_xyz || !d_out_intensities || !d_out_ids || !d_count)
+    return AMB_ERR_INVALID_ARGUMENT;
+  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
+  return dsm_extract_halo(ctx, d_xyz, reinterpret_cast<const unsigned long long*>(d_ids), n, y_lo, y_hi, reach, 0.0,
+                          d_out_xyz, reinterpret_cast<unsigned long long*>(d_out_ids), capacity, d_count, d_intensities,
+                          d_out_intensities);
 }
 
 int amb_ortho_from_pcl_process(amb_ctx* ctx, const double* xyz, const int32_t* intensities, size_t n,
@@ -413,11 +442,15 @@ int amb_ortho_from_pcl_process(amb_ctx* ctx, const double* xyz, const int32_t* i
   float* saved = nullptr;
   if (use_adaptive_interpolation) {
     const int pst = pcl_adaptive_prepare(ctx, &saved);
-    if (pst != AMB_OK) return pcl_adaptive_finish(ctx, pst, n, interpolation_radius, saved);
+    if (pst != AMB_OK)
+      return pcl_adaptive_finish(ctx, pst, ctx->points.as<double>(), nullptr, ctx->intensities.as<int>(), n,
+                                 interpolation_radius, saved);
   }
   int st = dsm_run(ctx, ctx->points.as<double>(), nullptr, n, interpolation_radius, 0.0, 0.0, 1,
                    ctx->intensities.as<int>());
-  if (use_adaptive_interpolation) st = pcl_adaptive_finish(ctx, st, n, interpolation_radius, saved);
+  if (use_adaptive_interpolation)
+    st = pcl_adaptive_finish(ctx, st, ctx->points.as<double>(), nullptr, ctx->intensities.as<int>(), n,
+                             interpolation_radius, saved);
   ctx->dsm_timed = (st == AMB_OK);
   if (st != AMB_OK) return st;
   AMB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));

@@ -1,5 +1,6 @@
 // amb_comm.cu — the one exchange step of the path inside the library (SURVEY.md §8e): a context can join an NCCL
-// communicator (one process per GPU, or several contexts of one process), and amb_dsm_process_sharded_device runs
+// communicator (one process per GPU, or several contexts of one process), and amb_dsm_process_sharded_device (and
+// amb_ortho_from_pcl_process_sharded_device, whose records carry the intensities as z) runs
 //     border-halo compaction  ->  ONE ncclAllGather of the halos  ->  binning over [own points | neighbours' halos]
 // entirely on the context's stream: no host synchronisation, no framework plumbing, device-side counts.
 //
@@ -107,11 +108,12 @@ __device__ __forceinline__ void halo_append(bool take, int lane, unsigned char* 
   }
 }
 
-__global__ void __launch_bounds__(256) dsm_halo_records_kernel(const double* __restrict__ xyz,
-                                                               const unsigned long long* __restrict__ ids, size_t n,
-                                                               double y_lo, double y_hi, double reach, double shift_y,
-                                                               unsigned char* seg_up, unsigned char* seg_down, bool split,
-                                                               unsigned int capacity) {
+// INTENSITIES (OrthoFromPcl): the record's z is double(intensities[t]), what that pass bins (ortho-from-pcl.cc:33)
+template <bool INTENSITIES>
+__device__ __forceinline__ void halo_records(const double* __restrict__ xyz, const int* __restrict__ intensities,
+                                             const unsigned long long* __restrict__ ids, size_t n, double y_lo,
+                                             double y_hi, double reach, double shift_y, unsigned char* seg_up,
+                                             unsigned char* seg_down, bool split, unsigned int capacity) {
   const int lane = threadIdx.x & 31;
   const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
   const size_t n_round = ((n + stride - 1) / stride) * stride;  // whole warps stay converged for the ballots
@@ -126,7 +128,7 @@ __global__ void __launch_bounds__(256) dsm_halo_records_kernel(const double* __r
       down = ys < y_lo + reach;
       if (up || down) {
         x = xyz[3 * t + 0];
-        z = xyz[3 * t + 2];
+        z = INTENSITIES ? static_cast<double>(intensities[t]) : xyz[3 * t + 2];
         id = ids ? ids[t] : static_cast<unsigned long long>(t);
       }
     }
@@ -137,6 +139,23 @@ __global__ void __launch_bounds__(256) dsm_halo_records_kernel(const double* __r
       halo_append(up || down, lane, seg_up, capacity, x, y, z, id);
     }
   }
+}
+
+__global__ void __launch_bounds__(256) dsm_halo_records_kernel(const double* __restrict__ xyz,
+                                                               const unsigned long long* __restrict__ ids, size_t n,
+                                                               double y_lo, double y_hi, double reach, double shift_y,
+                                                               unsigned char* seg_up, unsigned char* seg_down, bool split,
+                                                               unsigned int capacity) {
+  halo_records<false>(xyz, nullptr, ids, n, y_lo, y_hi, reach, shift_y, seg_up, seg_down, split, capacity);
+}
+
+__global__ void __launch_bounds__(256) pcl_halo_records_kernel(const double* __restrict__ xyz,
+                                                               const int* __restrict__ intensities,
+                                                               const unsigned long long* __restrict__ ids, size_t n,
+                                                               double y_lo, double y_hi, double reach,
+                                                               unsigned char* seg_up, unsigned char* seg_down, bool split,
+                                                               unsigned int capacity) {
+  halo_records<true>(xyz, intensities, ids, n, y_lo, y_hi, reach, 0.0, seg_up, seg_down, split, capacity);
 }
 
 
@@ -377,16 +396,16 @@ int amb_comm_last_exchange(const amb_ctx* ctx) { return ctx ? ctx->halo_last_exc
 int amb_comm_size(const amb_ctx* ctx) { return ctx ? ctx->comm_size : 0; }
 int amb_comm_rank(const amb_ctx* ctx) { return ctx ? ctx->comm_rank : -1; }
 
-int amb_dsm_process_sharded_device(amb_ctx* ctx, const double* d_xyz, const uint64_t* d_ids, size_t n_local,
-                                   int32_t interpolation_radius, double center_easting, double center_northing,
-                                   uint32_t halo_capacity) {
-  if (!ctx) return AMB_ERR_INVALID_ARGUMENT;
-  if (!d_xyz || !d_ids) return AMB_ERR_INVALID_ARGUMENT;  // a sharded cloud needs global ids
-  if (interpolation_radius < 1) return AMB_ERR_INVALID_ARGUMENT;
-  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
-  if (ctx->comm_size <= 1 || !ctx->nccl_comm)  // not sharded: the whole cloud is here
-    return amb_dsm_process_device_ids(ctx, d_xyz, d_ids, n_local, interpolation_radius, center_easting,
-                                      center_northing);
+}  // extern "C"
+
+namespace amb {
+
+// The sharded step shared by Dsm (mode 0) and OrthoFromPcl (mode 1, d_intensities: every record's z is the point's
+// intensity, no centre shift): exchange of the border halos, then the binning over [own points | neighbours' halos].
+// The caller has checked the arguments and that the context belongs to a communicator of several ranks.
+static int sharded_step(amb_ctx* ctx, const double* d_xyz, const int* d_intensities, const uint64_t* d_ids,
+                        size_t n_local, int32_t interpolation_radius, double center_easting, double center_northing,
+                        uint32_t halo_capacity, int mode) {
   if (halo_capacity == 0) return AMB_ERR_INVALID_ARGUMENT;
   const int nranks = ctx->comm_size, rank = ctx->comm_rank;
   const size_t seg_bytes = 32 * (static_cast<size_t>(halo_capacity) + 1);  // header + records
@@ -396,6 +415,18 @@ int amb_dsm_process_sharded_device(amb_ctx* ctx, const double* d_xyz, const uint
   int st = amb_stripe_y_interval(&ctx->geom, ctx->col_begin, ctx->col_end, &y_lo, &y_hi);
   if (st != AMB_OK) return st;
   const double reach = amb_dsm_halo_reach(&ctx->geom, interpolation_radius);
+  // compaction of this rank's border points into exchange segments (the NCCL exchanges; peer push compacts in the binning)
+  auto compact = [&](unsigned char* seg_up, unsigned char* seg_down, bool split, uint32_t capacity) {
+    if (n_local == 0) return cudaSuccess;
+    const unsigned long long* ids = reinterpret_cast<const unsigned long long*>(d_ids);
+    if (d_intensities)
+      pcl_halo_records_kernel<<<ctx->num_sms * 8, 256, 0, s>>>(d_xyz, d_intensities, ids, n_local, y_lo, y_hi, reach,
+                                                               seg_up, seg_down, split, capacity);
+    else
+      dsm_halo_records_kernel<<<ctx->num_sms * 8, 256, 0, s>>>(d_xyz, ids, n_local, y_lo, y_hi, reach, center_easting,
+                                                               seg_up, seg_down, split, capacity);
+    return cudaGetLastError();
+  };
 
   // Who needs this rank's border points?  If the stripes are consecutive (rank r + 1 starts where rank r ends) and every
   // stripe is at least `reach` wide, only the two adjacent ranks do: two ncclSend / ncclRecv pairs in one group move each
@@ -469,12 +500,7 @@ int amb_dsm_process_sharded_device(amb_ctx* ctx, const double* d_xyz, const uint
     AMB_CUDA(ctx, cudaMemsetAsync(send + side_bytes, 0, 32, s));
     AMB_CUDA(ctx, cudaMemsetAsync(recv, 0, 32, s));              // a missing neighbour contributes an empty list
     AMB_CUDA(ctx, cudaMemsetAsync(recv + side_bytes, 0, 32, s));
-    if (n_local > 0) {
-      dsm_halo_records_kernel<<<ctx->num_sms * 8, 256, 0, s>>>(
-          d_xyz, reinterpret_cast<const unsigned long long*>(d_ids), n_local, y_lo, y_hi, reach, center_easting, send,
-          send + side_bytes, true, side_capacity);
-      AMB_CUDA(ctx, cudaGetLastError());
-    }
+    AMB_CUDA(ctx, compact(send, send + side_bytes, true, side_capacity));
     nccl_comm_t comm = static_cast<nccl_comm_t>(ctx->nccl_comm);
     int rc = nccl().group_start();
     if (rc == 0 && rank > 0) rc = nccl().send(send, side_bytes, kNcclInt8, rank - 1, comm, s);
@@ -493,12 +519,7 @@ int amb_dsm_process_sharded_device(amb_ctx* ctx, const double* d_xyz, const uint
     AMB_CUDA(ctx, ctx->halo_recv.reserve(seg_bytes * nranks));
     unsigned char* send = ctx->halo_send.as<unsigned char>();
     AMB_CUDA(ctx, cudaMemsetAsync(send, 0, 32, s));
-    if (n_local > 0) {
-      dsm_halo_records_kernel<<<ctx->num_sms * 8, 256, 0, s>>>(
-          d_xyz, reinterpret_cast<const unsigned long long*>(d_ids), n_local, y_lo, y_hi, reach, center_easting, send,
-          send, false, halo_capacity);
-      AMB_CUDA(ctx, cudaGetLastError());
-    }
+    AMB_CUDA(ctx, compact(send, send, false, halo_capacity));
     // the one collective of the step
     const int rc = nccl().all_gather(send, ctx->halo_recv.ptr, seg_bytes, kNcclInt8,
                                      static_cast<nccl_comm_t>(ctx->nccl_comm), s);
@@ -511,9 +532,62 @@ int amb_dsm_process_sharded_device(amb_ctx* ctx, const double* d_xyz, const uint
   AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_H2D_END], s));  // "h2d" slot of the timings = the halo step
   ctx->dsm_had_h2d = true;
   st = dsm_run(ctx, d_xyz, reinterpret_cast<const unsigned long long*>(d_ids), n_local, interpolation_radius,
-               center_easting, center_northing, 0, nullptr, &halo, use_push ? &push : nullptr);
+               center_easting, center_northing, mode, d_intensities, &halo, use_push ? &push : nullptr);
   ctx->dsm_timed = (st == AMB_OK);
   return st;
+}
+
+}  // namespace amb
+
+extern "C" {
+
+int amb_dsm_process_sharded_device(amb_ctx* ctx, const double* d_xyz, const uint64_t* d_ids, size_t n_local,
+                                   int32_t interpolation_radius, double center_easting, double center_northing,
+                                   uint32_t halo_capacity) {
+  if (!ctx) return AMB_ERR_INVALID_ARGUMENT;
+  if (!d_xyz || !d_ids) return AMB_ERR_INVALID_ARGUMENT;  // a sharded cloud needs global ids
+  if (interpolation_radius < 1) return AMB_ERR_INVALID_ARGUMENT;
+  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
+  if (ctx->comm_size <= 1 || !ctx->nccl_comm)  // not sharded: the whole cloud is here
+    return amb_dsm_process_device_ids(ctx, d_xyz, d_ids, n_local, interpolation_radius, center_easting,
+                                      center_northing);
+  return sharded_step(ctx, d_xyz, nullptr, d_ids, n_local, interpolation_radius, center_easting, center_northing,
+                      halo_capacity, 0);
+}
+
+int amb_ortho_from_pcl_process_sharded_device(amb_ctx* ctx, const double* d_xyz, const int32_t* d_intensities,
+                                              const uint64_t* d_ids, size_t n_local, int32_t interpolation_radius,
+                                              uint32_t halo_capacity) {
+  if (!ctx) return AMB_ERR_INVALID_ARGUMENT;
+  if (!d_xyz || !d_intensities || !d_ids) return AMB_ERR_INVALID_ARGUMENT;  // a sharded cloud needs global ids
+  if (interpolation_radius < 1) return AMB_ERR_INVALID_ARGUMENT;
+  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
+  if (ctx->comm_size <= 1 || !ctx->nccl_comm)  // not sharded: the whole cloud is here
+    return amb_ortho_from_pcl_process_device_ids(ctx, d_xyz, d_intensities, d_ids, n_local, interpolation_radius, 0);
+  return sharded_step(ctx, d_xyz, d_intensities, d_ids, n_local, interpolation_radius, 0.0, 0.0, halo_capacity, 1);
+}
+
+int amb_ortho_from_pcl_process_sharded(amb_ctx* ctx, const double* xyz, const int32_t* intensities, const uint64_t* ids,
+                                       size_t n_local, int32_t interpolation_radius, uint32_t halo_capacity) {
+  if (!ctx || !xyz || !intensities || !ids) return AMB_ERR_INVALID_ARGUMENT;
+  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
+  AMB_CUDA(ctx, ctx->points.reserve(std::max<size_t>(n_local, 1) * 3 * sizeof(double)));
+  AMB_CUDA(ctx, ctx->intensities.reserve(std::max<size_t>(n_local, 1) * sizeof(int32_t)));
+  AMB_CUDA(ctx, ctx->point_ids.reserve(std::max<size_t>(n_local, 1) * sizeof(uint64_t)));
+  if (n_local) {
+    const int sst = staged_h2d(ctx, ctx->points.ptr, xyz, n_local * 3 * sizeof(double), ctx->stream);
+    if (sst != AMB_OK) return sst;
+    AMB_CUDA(ctx, cudaMemcpyAsync(ctx->intensities.ptr, intensities, n_local * sizeof(int32_t), cudaMemcpyHostToDevice,
+                                  ctx->stream));
+    AMB_CUDA(ctx, cudaMemcpyAsync(ctx->point_ids.ptr, ids, n_local * sizeof(uint64_t), cudaMemcpyHostToDevice,
+                                  ctx->stream));
+  }
+  const int st = amb_ortho_from_pcl_process_sharded_device(ctx, ctx->points.as<double>(), ctx->intensities.as<int32_t>(),
+                                                           ctx->point_ids.as<uint64_t>(), n_local, interpolation_radius,
+                                                           halo_capacity);
+  if (st != AMB_OK) return st;
+  AMB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // host entry points are synchronous (ortho final on the device)
+  return AMB_OK;
 }
 
 int amb_dsm_process_sharded(amb_ctx* ctx, const double* xyz, const uint64_t* ids, size_t n_local,

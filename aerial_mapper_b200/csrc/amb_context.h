@@ -198,7 +198,8 @@ struct amb_ctx {
   int dsm_precision = AMB_DSM_F32;  // amb_dsm_set_precision: arithmetic of the tile gather's weights and sums
   bool dsm_debug_valid = false;
   int64_t last_points_binned = 0, last_cells_empty = 0;
-  std::vector<unsigned char> last_dsm_plan;  // the DsmPlan of the last dsm_run (read by the adaptive OrthoFromPcl pass)
+  std::vector<unsigned char> last_dsm_plan;  // the DsmPlan of the last dsm_run (read by the adaptive OrthoFromPcl pass;
+                                             // on a stripe: of its whole-map binning, dsm_run(.., whole_map_bins))
 
   // Ortho scratch
   amb::DeviceBuffer frames;       // device copies of the caller's frames (host entry point)
@@ -259,13 +260,18 @@ int staged_h2d_rects(amb_ctx* ctx, const StagedRect* rects, size_t n, cudaStream
 // Implemented in dsm_kernels.cu / ortho_kernels.cu
 int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, size_t n,
             int32_t interpolation_radius, double center_easting, double center_northing, int mode = 0,
-            const int* d_intensities = nullptr, const HaloSource* halo = nullptr, const HaloPush* push = nullptr);
+            const int* d_intensities = nullptr, const HaloSource* halo = nullptr, const HaloPush* push = nullptr,
+            bool whole_map_bins = false);
+// d_intensities != nullptr (OrthoFromPcl): the halo's intensities go to d_out_intensities, no centre shift
 int dsm_extract_halo(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, size_t n, double y_lo,
                      double y_hi, double reach, double center_easting, double* d_out_xyz,
-                     unsigned long long* d_out_ids, unsigned int capacity, unsigned int* d_count);
-// Implemented in pcl_adaptive_kernels.cu: ortho::Settings::use_adaptive_interpolation around dsm_run(mode = 1)
+                     unsigned long long* d_out_ids, unsigned int capacity, unsigned int* d_count,
+                     const int* d_intensities = nullptr, int* d_out_intensities = nullptr);
+// Implemented in pcl_adaptive_kernels.cu: ortho::Settings::use_adaptive_interpolation around dsm_run(mode = 1).  On a
+// stripe, finish bins the same points (the whole cloud) again on the whole map's bin grid.
 int pcl_adaptive_prepare(amb_ctx* ctx, float** saved);
-int pcl_adaptive_finish(amb_ctx* ctx, int pass_status, size_t n, int32_t interpolation_radius, float* saved);
+int pcl_adaptive_finish(amb_ctx* ctx, int pass_status, const double* d_xyz, const unsigned long long* d_ids,
+                        const int* d_intensities, size_t n, int32_t interpolation_radius, float* saved);
 int ortho_run(amb_ctx* ctx, const amb_camera* camera, const double* T_G_B, const uint8_t* const* d_images,
               const uint8_t* const* h_images, size_t n, int32_t channels, size_t row_step, int32_t colored_ortho);
 std::vector<double> dsm_thresholds(int32_t interpolation_radius);

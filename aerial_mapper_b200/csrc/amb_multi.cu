@@ -9,6 +9,8 @@
 //            ARRIVES sharded uses the per-context amb_dsm_process_sharded* with its halo exchange.)
 //     ortho  every device evaluates its stripe over all frames; with host frames only the winners' sub-rectangles of the
 //            stripe cross that device's PCIe link.
+//     OrthoFromPcl  like DSM (whole cloud and intensities to every device); adaptive interpolation included, whose far
+//            thresholds read the whole cloud each device holds (pcl_adaptive_kernels.cu).
 //   Host layers are full column-major maps; a stripe is a contiguous range of them.
 // The blocking host entry points of the stripes run concurrently on one std::thread per device.
 #include <thread>
@@ -141,6 +143,22 @@ int amb_multi_dsm_process(amb_multi* m, const double* xyz, size_t n, int32_t int
   return for_each_stripe(m, [&](int, amb_ctx* c) {
     int st = amb_dsm_set_density_hint(c, per_cell);
     if (st == AMB_OK) st = amb_dsm_process(c, xyz, n, interpolation_radius, center_easting, center_northing);
+    return st;
+  });
+}
+
+int amb_multi_ortho_from_pcl_process(amb_multi* m, const double* xyz, const int32_t* intensities, size_t n,
+                                     int32_t interpolation_radius, int32_t use_adaptive_interpolation) {
+  if (!m) return AMB_ERR_INVALID_ARGUMENT;
+  if (n == 0) return AMB_ERR_EMPTY;  // CHECK(!pointcloud.empty()), ortho-from-pcl.cc:23
+  if (!xyz || !intensities) return AMB_ERR_INVALID_ARGUMENT;
+  // as amb_multi_dsm_process: the density of the WHOLE cloud fixes the bucket edge on every device, which the adaptive
+  // pass's whole-map binning also needs to visit the buckets of a single-GPU run
+  const double per_cell = static_cast<double>(n) / (static_cast<double>(m->geom.rows) * static_cast<double>(m->geom.cols));
+  return for_each_stripe(m, [&](int, amb_ctx* c) {
+    int st = amb_dsm_set_density_hint(c, per_cell);
+    if (st == AMB_OK)
+      st = amb_ortho_from_pcl_process(c, xyz, intensities, n, interpolation_radius, use_adaptive_interpolation);
     return st;
   });
 }

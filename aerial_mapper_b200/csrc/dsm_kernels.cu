@@ -651,22 +651,26 @@ inline int round_up(int v, int m) { return ((v + m - 1) / m) * m; }
 // Points of a sharded cloud that lie within `reach` of the borders of the y-interval (y_lo, y_hi] a rank owns:
 // what its neighbours need for interpolation (the "border halo").  Unordered append (warp-aggregated atomic);
 // order does not matter because every point carries its global id.
-__global__ void __launch_bounds__(256) dsm_halo_kernel(const double* __restrict__ xyz,
-                                                       const unsigned long long* __restrict__ ids, size_t n,
-                                                       double y_lo, double y_hi, double reach, double shift_y,
-                                                       double* __restrict__ out_xyz,
-                                                       unsigned long long* __restrict__ out_ids,
-                                                       unsigned int capacity, unsigned int* __restrict__ count) {
+// INTENSITIES (OrthoFromPcl): each point's intensity travels beside its coordinates.
+template <bool INTENSITIES>
+__device__ __forceinline__ void halo_compact(const double* __restrict__ xyz, const int* __restrict__ intensities,
+                                             const unsigned long long* __restrict__ ids, size_t n, double y_lo,
+                                             double y_hi, double reach, double shift_y, double* __restrict__ out_xyz,
+                                             int* __restrict__ out_intensities,
+                                             unsigned long long* __restrict__ out_ids, unsigned int capacity,
+                                             unsigned int* __restrict__ count) {
   const int lane = threadIdx.x & 31;
   const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
   const size_t n_round = ((n + stride - 1) / stride) * stride;  // whole warps stay converged for the ballot
   for (size_t t = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; t < n_round; t += stride) {
     bool take = false;
     double x = 0, y = 0, z = 0;
+    int v = 0;
     if (t < n) {
       x = xyz[3 * t + 0];
       y = xyz[3 * t + 1];
       z = xyz[3 * t + 2];
+      if (INTENSITIES) v = intensities[t];
       const double ys = y - shift_y;
       take = (ys < y_lo + reach) || (ys > y_hi - reach);
     }
@@ -682,6 +686,7 @@ __global__ void __launch_bounds__(256) dsm_halo_kernel(const double* __restrict_
           out_xyz[3 * static_cast<size_t>(slot) + 0] = x;
           out_xyz[3 * static_cast<size_t>(slot) + 1] = y;
           out_xyz[3 * static_cast<size_t>(slot) + 2] = z;
+          if (INTENSITIES) out_intensities[slot] = v;
           out_ids[slot] = ids ? ids[t] : static_cast<unsigned long long>(t);
         }
       }
@@ -689,21 +694,52 @@ __global__ void __launch_bounds__(256) dsm_halo_kernel(const double* __restrict_
   }
 }
 
+__global__ void __launch_bounds__(256) dsm_halo_kernel(const double* __restrict__ xyz,
+                                                       const unsigned long long* __restrict__ ids, size_t n,
+                                                       double y_lo, double y_hi, double reach, double shift_y,
+                                                       double* __restrict__ out_xyz,
+                                                       unsigned long long* __restrict__ out_ids,
+                                                       unsigned int capacity, unsigned int* __restrict__ count) {
+  halo_compact<false>(xyz, nullptr, ids, n, y_lo, y_hi, reach, shift_y, out_xyz, nullptr, out_ids, capacity, count);
+}
+
+__global__ void __launch_bounds__(256) pcl_halo_kernel(const double* __restrict__ xyz,
+                                                       const int* __restrict__ intensities,
+                                                       const unsigned long long* __restrict__ ids, size_t n,
+                                                       double y_lo, double y_hi, double reach,
+                                                       double* __restrict__ out_xyz, int* __restrict__ out_intensities,
+                                                       unsigned long long* __restrict__ out_ids,
+                                                       unsigned int capacity, unsigned int* __restrict__ count) {
+  halo_compact<true>(xyz, intensities, ids, n, y_lo, y_hi, reach, 0.0, out_xyz, out_intensities, out_ids, capacity,
+                     count);
+}
+
 int dsm_extract_halo(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, size_t n, double y_lo,
                      double y_hi, double reach, double center_easting, double* d_out_xyz,
-                     unsigned long long* d_out_ids, unsigned int capacity, unsigned int* d_count) {
+                     unsigned long long* d_out_ids, unsigned int capacity, unsigned int* d_count,
+                     const int* d_intensities, int* d_out_intensities) {
   AMB_CUDA(ctx, cudaMemsetAsync(d_count, 0, sizeof(unsigned int), ctx->stream));
-  dsm_halo_kernel<<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(d_xyz, d_ids, n, y_lo, y_hi, reach, center_easting,
-                                                             d_out_xyz, d_out_ids, capacity, d_count);
+  if (d_intensities)  // OrthoFromPcl: no centre shift (ortho-from-pcl.cc bins the raw coordinates)
+    pcl_halo_kernel<<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(d_xyz, d_intensities, d_ids, n, y_lo, y_hi, reach,
+                                                               d_out_xyz, d_out_intensities, d_out_ids, capacity,
+                                                               d_count);
+  else
+    dsm_halo_kernel<<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(d_xyz, d_ids, n, y_lo, y_hi, reach, center_easting,
+                                                               d_out_xyz, d_out_ids, capacity, d_count);
   AMB_CUDA(ctx, cudaGetLastError());
   return AMB_OK;
 }
 
 int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, size_t n,
             int32_t interpolation_radius, double center_easting, double center_northing, int mode,
-            const int* d_intensities, const HaloSource* halo, const HaloPush* push) {
+            const int* d_intensities, const HaloSource* halo, const HaloPush* push, bool whole_map_bins) {
   const amb_geometry& g = ctx->geom;
   if (n == 0 && !halo) return AMB_ERR_EMPTY;
+  // whole_map_bins (adaptive OrthoFromPcl on a stripe, pcl_adaptive_kernels.cu): bin the points into the bin grid of a
+  // context owning the whole map — same bucket edge, same global bucket lattice — and stop after the binning.  The plan
+  // left in last_dsm_plan keeps that grid but names this stripe's first column and width, so that its cells map into it.
+  const int32_t col_begin = whole_map_bins ? 0 : ctx->col_begin;
+  const int32_t col_end = whole_map_bins ? g.cols : ctx->col_end;
   const size_t n_own = n;
   // with halos: [own points | padding to a whole tile | halo slots] — an upper bound of the records this rank bins
   if (halo) n = ((n_own + 2047) / 2048) * 2048 + static_cast<size_t>(halo->nranks) * halo->capacity;
@@ -729,8 +765,8 @@ int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, 
   plan.n_thr = static_cast<int>(thr.size());
   plan.thr0 = static_cast<double>(interpolation_radius);
   plan.rows = g.rows;
-  plan.cols_slab = ctx->col_end - ctx->col_begin;
-  plan.col_begin = ctx->col_begin;
+  plan.cols_slab = col_end - col_begin;
+  plan.col_begin = col_begin;
   plan.res = g.resolution;
   plan.inv_res = 1.0 / g.resolution;
   plan.base_x = g.pos_x + (0.5 * g.length_x - 0.5 * g.resolution);
@@ -763,8 +799,8 @@ int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, 
   plan.Pa = round_up(plan.P, B);
   // Tiles align to GLOBAL columns (multiples of TJ), so that the content of a tile — hence the shared-memory /
   // warp-per-cell path decision and every summation order — does not depend on how the map is striped.
-  plan.tile_j0 = ctx->col_begin / TJ;
-  const int tile_j1 = (ctx->col_end - 1) / TJ;  // last tile column (inclusive)
+  plan.tile_j0 = col_begin / TJ;
+  const int tile_j1 = (col_end - 1) / TJ;  // last tile column (inclusive)
   plan.gj0 = plan.tile_j0 * TJ - plan.Pa;
   plan.BR = round_up(round_up(g.rows, TI) + 2 * plan.Pa, B);
   plan.BC = round_up((tile_j1 + 1) * TJ + plan.Pa - plan.gj0, B);
@@ -799,11 +835,11 @@ int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, 
   // only this stage's own slots: the sticky CHECK flags of earlier asynchronous calls stay until they are reported
   AMB_CUDA(ctx, cudaMemsetAsync(counters + CTR_DSM_LIST, 0, sizeof(unsigned int), s));
   AMB_CUDA(ctx, cudaMemsetAsync(counters + CTR_DSM_BINNED, 0, 4 * sizeof(unsigned int), s));  // [2..5]
-  if (ctx->dsm_debug) {
+  if (ctx->dsm_debug && !whole_map_bins) {
     AMB_CUDA(ctx, cudaMemsetAsync(ctx->dbg_count.ptr, 0xff, cells * sizeof(int), s));
     AMB_CUDA(ctx, cudaMemsetAsync(ctx->dbg_level.ptr, 0xff, cells, s));
   }
-  ctx->dsm_launches = 0;
+  if (!whole_map_bins) ctx->dsm_launches = 0;
 
   const int stream_grid = ctx->num_sms * 8;
   const HaloSource hs = halo ? *halo : HaloSource();
@@ -876,6 +912,14 @@ int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, 
     ctx->dsm_launches += 1;
   }
   ctx->dsm_launches += 5;
+  if (whole_map_bins) {
+    AMB_CUDA(ctx, cudaGetLastError());
+    plan.col_begin = ctx->col_begin;
+    plan.cols_slab = ctx->col_end - ctx->col_begin;
+    ctx->last_dsm_plan.assign(reinterpret_cast<const unsigned char*>(&plan),
+                              reinterpret_cast<const unsigned char*>(&plan) + sizeof(plan));
+    return AMB_OK;
+  }
   AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_BIN_END], s));
 
   // gather

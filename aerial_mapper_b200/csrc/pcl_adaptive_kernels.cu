@@ -15,9 +15,14 @@
 //             (pcl_adaptive_cell_kernel) straight from the bucket records the pass left in HBM — per level the
 //             smallest d2 over the window the threshold can reach, then the IDW over d2 < threshold, visiting
 //             records through order[] (canonical order) exactly like dsm_cell_kernel does for the DSM's retry loop.
-// Restrictions (AMB_ERR_UNSUPPORTED, layer restored): the context must own the whole map (a stripe does not hold the
-// far points an unbounded radius may need) and every point must lie inside the map's bin grid (map + apron), because
-// the binning drops what lies outside; radius growth beyond `int` range is undefined behaviour in the reference.
+// On a stripe (a context owning columns [col_begin, col_end) that is passed the WHOLE cloud, as amb_multi does) the
+// regular pass bins only what reaches the stripe, while a far threshold may need any point.  finish therefore bins the
+// cloud again with the plan a whole-map context builds (same density, hence the same bucket edge; the same global
+// bucket lattice, tile_j0 = 0) and maps the stripe's cells into that grid (plan.col_begin = the stripe's first column,
+// gj0 = the whole map's): every cell visits the same buckets in the same order with the same lane split as in the
+// whole-map run, so the stripe is bit-identical to those columns.  A whole-map context reuses the regular pass's bins.
+// Restrictions (AMB_ERR_UNSUPPORTED, layer restored): every point must lie inside the map's bin grid (map + apron),
+// because the binning drops what lies outside; radius growth beyond `int` range is undefined behaviour in the reference.
 #include <cfloat>
 #include <climits>
 #include <cmath>
@@ -133,10 +138,6 @@ __global__ void __launch_bounds__(256) pcl_adaptive_cell_kernel(const __grid_con
 // pcl_adaptive_finish) and filled with the NaN sentinel.
 int pcl_adaptive_prepare(amb_ctx* ctx, float** saved) {
   *saved = nullptr;
-  if (ctx->col_begin != 0 || ctx->col_end != ctx->geom.cols) {
-    ctx->last_error = "adaptive interpolation needs a context that owns the whole map";
-    return AMB_ERR_UNSUPPORTED;
-  }
   int st = ensure_layer(ctx, AMB_LAYER_ORTHO);
   if (st != AMB_OK) return st;
   wait_layer_copy(ctx, AMB_LAYER_ORTHO);
@@ -148,7 +149,8 @@ int pcl_adaptive_prepare(amb_ctx* ctx, float** saved) {
 }
 
 // After the regular pass (`pass_status` = what dsm_run returned).  On any failure the slab gets its saved content back.
-int pcl_adaptive_finish(amb_ctx* ctx, int pass_status, size_t n, int32_t interpolation_radius, float* saved) {
+int pcl_adaptive_finish(amb_ctx* ctx, int pass_status, const double* d_xyz, const unsigned long long* d_ids,
+                        const int* d_intensities, size_t n, int32_t interpolation_radius, float* saved) {
   const size_t cells = ctx->slab_cells();
   const size_t bytes = cells * sizeof(float);
   float* ortho = ctx->layers[AMB_LAYER_ORTHO];
@@ -163,6 +165,10 @@ int pcl_adaptive_finish(amb_ctx* ctx, int pass_status, size_t n, int32_t interpo
     return status;
   };
   if (pass_status != AMB_OK) return restore(pass_status);
+  if (ctx->col_begin != 0 || ctx->col_end != ctx->geom.cols) {  // a stripe: the whole map's bins (see the file header)
+    const int st = dsm_run(ctx, d_xyz, d_ids, n, interpolation_radius, 0.0, 0.0, 1, d_intensities, nullptr, nullptr, true);
+    if (st != AMB_OK) return restore(st);
+  }
   if (ctx->last_dsm_plan.size() != sizeof(DsmPlan)) return restore(AMB_ERR_INVALID_ARGUMENT);
   DsmPlan plan;
   std::memcpy(&plan, ctx->last_dsm_plan.data(), sizeof(plan));

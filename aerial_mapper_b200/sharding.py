@@ -99,20 +99,29 @@ class HaloExchange(object):
 
     send buffer (float64): [xyz: 3*cap | ids: cap (uint64 bits) | count: 1]; one all-gather fills `gathered`
     [world, 4*cap + 1]; assemble() lays out the DSM input `big_xyz` / `big_ids` = [all halos | local points] with
-    this rank's own halo slot and every unused slot set to NaN (amb's binning drops NaN points)."""
+    this rank's own halo slot and every unused slot set to NaN (amb's binning drops NaN points).
+    With `local_intensities` (OrthoFromPcl) the send buffer carries them too, as int32 bits in ceil(cap/2) more
+    float64 slots after the count, and assemble() also lays out `big_intensities` beside `big_xyz` / `big_ids`."""
 
-    def __init__(self, torch, world, rank, cap, local_xyz, local_ids, device):
+    def __init__(self, torch, world, rank, cap, local_xyz, local_ids, device, local_intensities=None):
         self.torch, self.world, self.rank, self.cap = torch, world, rank, int(cap)
         n = local_xyz.shape[0]
         self.n_local = n
-        self.send = torch.empty(4 * self.cap + 1, dtype=torch.float64, device=device)
-        self.gathered = torch.empty((world, 4 * self.cap + 1), dtype=torch.float64, device=device)
+        self.with_intensities = local_intensities is not None
+        row = 4 * self.cap + 1 + ((self.cap + 1) // 2 if self.with_intensities else 0)
+        self.send = torch.empty(row, dtype=torch.float64, device=device)
+        self.gathered = torch.empty((world, row), dtype=torch.float64, device=device)
         self.big_xyz = torch.empty((world * self.cap + n, 3), dtype=torch.float64, device=device)
         self.big_ids = torch.empty(world * self.cap + n, dtype=torch.int64, device=device)
         self.big_xyz[world * self.cap:] = local_xyz
         self.big_ids[world * self.cap:] = local_ids
         self.local_xyz = self.big_xyz[world * self.cap:]
         self.local_ids = self.big_ids[world * self.cap:]
+        self.big_intensities = self.local_intensities = None
+        if self.with_intensities:
+            self.big_intensities = torch.zeros(world * self.cap + n, dtype=torch.int32, device=device)
+            self.big_intensities[world * self.cap:] = local_intensities
+            self.local_intensities = self.big_intensities[world * self.cap:]
         self.n_total = world * self.cap + n
 
     def use_stream(self, stream):
@@ -136,11 +145,20 @@ class HaloExchange(object):
         if not shared:
             self._host_sync()
         base = self.send.data_ptr()
-        check(lib().amb_dsm_extract_halo(ctx, C.c_void_p(self.local_xyz.data_ptr()),
-                                         C.c_void_p(self.local_ids.data_ptr()), self.n_local, float(y_lo),
-                                         float(y_hi), float(reach), float(center_easting), C.c_void_p(base),
-                                         C.c_void_p(base + 8 * 3 * self.cap), self.cap,
-                                         C.c_void_p(base + 8 * 4 * self.cap)), ctx)
+        if self.with_intensities:   # OrthoFromPcl: no centre shift
+            check(lib().amb_ortho_from_pcl_extract_halo(ctx, C.c_void_p(self.local_xyz.data_ptr()),
+                                                        C.c_void_p(self.local_intensities.data_ptr()),
+                                                        C.c_void_p(self.local_ids.data_ptr()), self.n_local,
+                                                        float(y_lo), float(y_hi), float(reach), C.c_void_p(base),
+                                                        C.c_void_p(base + 8 * (4 * self.cap + 1)),
+                                                        C.c_void_p(base + 8 * 3 * self.cap), self.cap,
+                                                        C.c_void_p(base + 8 * 4 * self.cap)), ctx)
+        else:
+            check(lib().amb_dsm_extract_halo(ctx, C.c_void_p(self.local_xyz.data_ptr()),
+                                             C.c_void_p(self.local_ids.data_ptr()), self.n_local, float(y_lo),
+                                             float(y_hi), float(reach), float(center_easting), C.c_void_p(base),
+                                             C.c_void_p(base + 8 * 3 * self.cap), self.cap,
+                                             C.c_void_p(base + 8 * 4 * self.cap)), ctx)
         if not shared:
             check(lib().amb_sync(ctx), ctx)
 
@@ -153,6 +171,9 @@ class HaloExchange(object):
         with self._on_stream():
             self.big_xyz[:w * cap] = self.gathered[:, :3 * cap].reshape(w * cap, 3)
             self.big_ids[:w * cap] = self.gathered[:, 3 * cap:4 * cap].reshape(-1).view(self.torch.int64)
+            if self.with_intensities:
+                packed = self.gathered[:, 4 * cap + 1:].contiguous().view(self.torch.int32)   # [w, 2 * ceil(cap/2)]
+                self.big_intensities[:w * cap] = packed[:, :cap].reshape(-1)
             self.big_xyz[self.rank * cap:(self.rank + 1) * cap] = float("nan")  # own halo: already local
         if getattr(self, "stream", None) is None:
             self._host_sync()

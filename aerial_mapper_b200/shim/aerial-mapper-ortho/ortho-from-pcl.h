@@ -31,13 +31,12 @@ class OrthoFromPcl {
     CHECK(map);
     CHECK(intensities.size() >= pointcloud.size());  // CHECK(i < intensities.size()) for every i, :32
     static_assert(sizeof(int) == sizeof(int32_t), "int32 intensities expected");
-    amb_ctx* ctx = context_->get(*map);
+    context_->get(*map);
     context_->upload(map, "ortho", AMB_LAYER_ORTHO);  // cells without neighbours keep their value
-    amb_shim::checkStatus(
-        amb_ortho_from_pcl_process(ctx, &pointcloud[0](0), reinterpret_cast<const int32_t*>(intensities.data()),
-                                   pointcloud.size(), settings_.interpolation_radius,
-                                   settings_.use_adaptive_interpolation ? 1 : 0),
-        ctx, "amb_ortho_from_pcl_process");
+    // one GPU, or the map's column stripes over AMB_SHIM_GPUS=N GPUs (amb_multi_ortho_from_pcl_process)
+    context_->orthoFromPclProcess(&pointcloud[0](0), reinterpret_cast<const int32_t*>(intensities.data()),
+                                  pointcloud.size(), settings_.interpolation_radius,
+                                  settings_.use_adaptive_interpolation ? 1 : 0);
     context_->download(map, "ortho", AMB_LAYER_ORTHO);
   }
 

@@ -190,6 +190,16 @@ class Context {
       checkStatus(amb_ortho_process(b_->ctx, cam, poses, rasters, n, channels, row_step, colored), b_->ctx, "amb_ortho_process");
     }
   }
+  void orthoFromPclProcess(const double* xyz, const int32_t* intensities, size_t n, int32_t radius, int32_t adaptive) {
+    b_->device_equals[AMB_LAYER_ORTHO] = nullptr;
+    if (b_->multi) {
+      checkMulti(amb_multi_ortho_from_pcl_process(b_->multi, xyz, intensities, n, radius, adaptive),
+                 "amb_multi_ortho_from_pcl_process");
+    } else {
+      checkStatus(amb_ortho_from_pcl_process(b_->ctx, xyz, intensities, n, radius, adaptive), b_->ctx,
+                  "amb_ortho_from_pcl_process");
+    }
+  }
   // (ortho-from-pcl.h) the output layer of OrthoFromPcl changed on the device
   void invalidate(int id) { b_->device_equals[id] = nullptr; }
 

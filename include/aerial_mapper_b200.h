@@ -267,13 +267,41 @@ int amb_dsm_thresholds(int32_t interpolation_radius, double* thresholds, int32_t
  * a zero-distance point taken as a "perfect match" (:90-96) instead of a CHECK failure.  Cells without a neighbour
  * keep their value.  use_adaptive_interpolation != 0 (:63-72, off in the demo's flag file): a cell whose primary
  * ball is empty takes the IDW over the first non-empty ball of the thresholds 10*r, 100*r, 1000*r, ... (`int`
- * arithmetic in the reference, defined while 10^k * r <= INT_MAX), so every cell gets a value.  That mode needs a
- * context owning the whole map and every point inside the map's bin grid (map + the apron of the search radius);
- * otherwise AMB_ERR_UNSUPPORTED and the layer keeps its content. */
+ * arithmetic in the reference, defined while 10^k * r <= INT_MAX), so every cell gets a value.  That mode needs the
+ * WHOLE cloud in the call (on a stripe context too: the stripe then bins it a second time on the whole map's bin grid,
+ * and amb_get_timings reports the points of that binning) and every point inside the map's bin grid (map + the apron
+ * of the search radius); otherwise AMB_ERR_UNSUPPORTED and the layer keeps its content.
+ * A stripe context gives, bit for bit, the same columns of the undivided map in both modes. */
 int amb_ortho_from_pcl_process(amb_ctx* ctx, const double* xyz, const int32_t* intensities, size_t n,
                                int32_t interpolation_radius, int32_t use_adaptive_interpolation);
 int amb_ortho_from_pcl_process_device(amb_ctx* ctx, const double* d_xyz, const int32_t* d_intensities, size_t n,
                                       int32_t interpolation_radius, int32_t use_adaptive_interpolation);
+/* ---- OrthoFromPcl on a cloud that arrives sharded by column stripe (multi-GPU; ortho-from-pcl.cc:20-113) ----
+ * The counterparts of the DSM's sharded entry points above, with every point's intensity beside it.  Bit-identical to
+ * the undivided map when every rank passes the same amb_dsm_set_density_hint.
+ * _device_ids: d_ids (global ids < 2^32, unique over the whole cloud) replace the array position as the canonical
+ * summation-order key, like amb_dsm_process_device_ids. */
+int amb_ortho_from_pcl_process_device_ids(amb_ctx* ctx, const double* d_xyz, const int32_t* d_intensities,
+                                          const uint64_t* d_ids, size_t n, int32_t interpolation_radius,
+                                          int32_t use_adaptive_interpolation);
+/* amb_dsm_extract_halo with the intensities: the border halo's points, intensities and ids (d_ids may be NULL: array
+ * positions) go to d_out_*; no centre shift.  Use the reach of amb_dsm_halo_reach (its thresholds include OrthoFromPcl's
+ * single radius; extra halo points change no bit).  *d_count may exceed capacity (truncated halo).  Asynchronous. */
+int amb_ortho_from_pcl_extract_halo(amb_ctx* ctx, const double* d_xyz, const int32_t* d_intensities,
+                                    const uint64_t* d_ids, size_t n, double y_lo, double y_hi, double reach,
+                                    double* d_out_xyz, int32_t* d_out_intensities, uint64_t* d_out_ids,
+                                    uint32_t capacity, uint32_t* d_count);
+/* amb_dsm_process_sharded_device for OrthoFromPcl: the same exchange step (amb_comm_set_exchange, reported by
+ * amb_comm_last_exchange; the records carry z = double(intensity)), then the stripe's `ortho`.  No adaptive mode: no rank
+ * holds the whole cloud.  Collective; without a communicator (or with one rank) it is
+ * amb_ortho_from_pcl_process_device_ids. */
+int amb_ortho_from_pcl_process_sharded_device(amb_ctx* ctx, const double* d_xyz, const int32_t* d_intensities,
+                                              const uint64_t* d_ids, size_t n_local, int32_t interpolation_radius,
+                                              uint32_t halo_capacity);
+/* Same with this rank's points, intensities and ids in HOST memory; returns when the stripe's `ortho` is final on the
+ * device. */
+int amb_ortho_from_pcl_process_sharded(amb_ctx* ctx, const double* xyz, const int32_t* intensities, const uint64_t* ids,
+                                       size_t n_local, int32_t interpolation_radius, uint32_t halo_capacity);
 
 /* ---- "next" row N3: stereo::Densifier::computePointCloud (aerial_mapper_dense_pcl/src/densifier.cpp:25-108) ----
  * Disparity map -> world points, the step right before Dsm::process in the incremental pipeline
@@ -365,6 +393,10 @@ int amb_multi_dsm_process(amb_multi* m, const double* xyz, size_t n, int32_t int
                           double center_easting, double center_northing);
 int amb_multi_ortho_process(amb_multi* m, const amb_camera* camera, const double* T_G_B, const uint8_t* const* images,
                             size_t n, int32_t channels, size_t row_step, int32_t colored_ortho);
+/* ortho::OrthoFromPcl::process (ortho-from-pcl.cc:20-113): like amb_multi_dsm_process, every device gets the whole cloud
+ * with its intensities and the density n / (rows * cols); adaptive interpolation included. */
+int amb_multi_ortho_from_pcl_process(amb_multi* m, const double* xyz, const int32_t* intensities, size_t n,
+                                     int32_t interpolation_radius, int32_t use_adaptive_interpolation);
 
 /* ---- measurement ---- */
 int amb_get_timings(amb_ctx* ctx, amb_timings* out);
