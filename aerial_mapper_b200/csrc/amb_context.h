@@ -96,7 +96,7 @@ enum CounterSlot {
   CTR_DSM_DENSE = 3,       // tiles handed whole to the warp-per-cell kernel
   CTR_DSM_LIST_DONE = 5,   // chunked evaluation: list lengths of the chunks already evaluated
   CTR_HALO_OVERFLOW = 6,   // sticky: a rank's border halo did not fit the capacity passed to amb_dsm_process_sharded_device
-  CTR_DSM_AMBIGUOUS = 4,   // f32 gather: cells re-evaluated exactly because a pair fell inside the guard band
+  CTR_DSM_AMBIGUOUS = 4,   // f32 gather: cells re-evaluated exactly (a pair inside the guard band, an unbounded height)
   CTR_ORTHO_CHECK = 8,     // sticky: CHECK(alpha > 0.0), ortho-backward-grid.cc:178
   CTR_PCL_CELLS = 10,      // adaptive OrthoFromPcl: cells listed for the 10^k radius growth
   CTR_PCL_UNRESOLVED = 11, // adaptive OrthoFromPcl: cells no level could fill

@@ -939,6 +939,9 @@ int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, 
     plan.thr_f = static_cast<float>(plan.thr0);
     plan.eps_f = static_cast<float>(2.0 * bound);
     plan.zrange_limit = 4096.0;
+    // the same rounding as a distance vector: |d(dx)|, |d(dy)| <= 2uM + u |d_f|  =>  |v_f - v| <= 2 sqrt(2) u M + u |v_f|
+    plan.hdelta = static_cast<float>(2.0 * std::sqrt(2.0) * u * M * (1.0 + 1e-6));
+    plan.hden_max = static_cast<float>(std::pow((0.01 - u) / (plan.hdelta * (1.0 + 3.0 * u)), 2.0) * (1.0 - 1e-6));
   }
   // Stage size: 1.6x the expected number of points in a tile window under a uniform density (the tail of a
   // Poisson count is far inside that; denser tiles go to the warp-per-cell kernel), clamped to [24 KB, 100 KB]

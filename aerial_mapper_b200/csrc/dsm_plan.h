@@ -47,6 +47,8 @@ struct DsmPlan {
   float thr_f;          // (float)thr0 — an int, exact
   float eps_f;          // |d2_f32 - d2_reference| <= eps_f for every pair a tile can stage (see dsm_run)
   double zrange_limit;  // tiles whose staged heights span more than this go to the all-FP64 kernel
+  float hdelta;         // |(dx_f, dy_f) - (dx, dy)| <= hdelta + u |(dx_f, dy_f)| for every staged pair (height bound)
+  float hden_max;       // hdelta sqrt(den) (1 + 3u) + u <= 0.01  <=>  den <= hden_max
 };
 
 __device__ __forceinline__ double cell_x(const DsmPlan& p, int i) {

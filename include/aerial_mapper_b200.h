@@ -193,8 +193,11 @@ int amb_dsm_set_density_hint(amb_ctx* ctx, double points_per_cell);
 /* Arithmetic of the tile gather's IDW weights and sums.  Neighbour SETS (d2 < threshold), retry levels and the NaN mask
  * are the reference's exact double-precision decisions in both modes.
  *   AMB_DSM_F32 (default): weights 1/d2 and both sums in float32 from tile-local coordinates and heights; any cell with a
- *       (cell, point) pair too close to the decision boundary for float32 to decide is re-evaluated in double.  Heights
- *       differ from the reference by far less than the 1e-4 relative the task allows (in practice <= 1 float32 ulp).
+ *       (cell, point) pair too close to the decision boundary for float32 to decide is re-evaluated in double, and so is
+ *       any cell whose float32 height a rounding-error bound cannot place within 1e-4 relative of the reference's (a
+ *       point close to the cell centre among contrasting heights, a tile height offset far from the cell's heights;
+ *       DESIGN.md §4.1).  Every height is therefore within 1e-4 relative of the reference's; on terrain-like clouds
+ *       almost all are within 1 float32 ulp.
  *   AMB_DSM_F64: everything in double in the reference's operation order (<= 1 float32 ulp by construction; ~2x slower). */
 typedef enum amb_dsm_precision { AMB_DSM_F64 = 0, AMB_DSM_F32 = 1 } amb_dsm_precision;
 int amb_dsm_set_precision(amb_ctx* ctx, int precision);

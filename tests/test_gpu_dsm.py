@@ -5,7 +5,9 @@ Bars: neighbour counts, retry-threshold indices and the NaN mask are integer-exa
 (amb_dsm_set_precision; the whole module runs once per mode, AMB_DSM_PRECISION):
   f64  elevation <= 1 float32 ulp from the oracle (bit-identical up to double summation order)
   f32  (library default) float32 weights / sums from tile-local coordinates: elevation within 1e-6 relative and <= 4 ulp
-       (north_star allows 1e-4 relative); measured: > 99.9 % of the cells bit-identical to the f64 mode."""
+       on these terrain-like clouds.  The library guarantees 1e-4 relative in every cell: a cell whose float32 height a
+       rounding-error bound cannot place within it is evaluated in double (test_gpu_dsm_heights.py tests that bound
+       where float32 fails).  Measured: > 99.9 % of the cells bit-identical to the f64 mode."""
 import ctypes as C
 import os
 
