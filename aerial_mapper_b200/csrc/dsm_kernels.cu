@@ -871,13 +871,17 @@ int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, 
     unsigned short* offs = ctx->tile_offsets.as<unsigned short>();
     const unsigned int own_tiles = static_cast<unsigned int>(pp.halo_base / kPartTile);
     const unsigned int max_grid = static_cast<unsigned int>(ctx->num_sms) * 4u;
+    AMB_CUDA(ctx, cudaFuncSetAttribute(dsm_partition_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       kPartStageBytes));
     if (push) {
       // peer-push exchange (amb_comm.cu): the own points are binned first and their border records stored into the
       // adjacent ranks' segments on the way; the incoming halos — the tiles after halo_base — follow once both neighbours
       // have published theirs.  (At least one block even without own points: it publishes the empty lists.)
       pp.tile_begin = 0;
       pp.tile_end = own_tiles;
-      dsm_partition_kernel<true><<<std::max(1u, std::min(own_tiles, max_grid)), kPartThreads, 0, s>>>(
+      AMB_CUDA(ctx, cudaFuncSetAttribute(dsm_partition_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         kPartStageBytes));
+      dsm_partition_kernel<true><<<std::max(1u, std::min(own_tiles, max_grid)), kPartThreads, kPartStageBytes, s>>>(
           d_xyz, d_intensities, d_ids, plan, pp, G, tmp, offs, counters, hs, *push);
       st = halo_wait_launch(ctx, *push);
       if (st != AMB_OK) return st;
@@ -886,13 +890,13 @@ int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, 
       pp.tile_begin = own_tiles;
       pp.tile_end = pp.n_tiles;
       if (pp.tile_end > pp.tile_begin)
-        dsm_partition_kernel<false><<<std::min(pp.tile_end - pp.tile_begin, max_grid), kPartThreads, 0, s>>>(
+        dsm_partition_kernel<false><<<std::min(pp.tile_end - pp.tile_begin, max_grid), kPartThreads, kPartStageBytes, s>>>(
             d_xyz, d_intensities, d_ids, plan, pp, G, tmp, offs, counters, hs, HaloPush());
       ctx->dsm_launches += 2;
     } else {
       pp.tile_begin = 0;
       pp.tile_end = pp.n_tiles;
-      dsm_partition_kernel<false><<<std::min(pp.n_tiles, max_grid), kPartThreads, 0, s>>>(
+      dsm_partition_kernel<false><<<std::min(pp.n_tiles, max_grid), kPartThreads, kPartStageBytes, s>>>(
           d_xyz, d_intensities, d_ids, plan, pp, G, tmp, offs, counters, hs, HaloPush());
     }
   }

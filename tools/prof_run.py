@@ -8,7 +8,8 @@ import aerial_mapper_b200 as amb
 from aerial_mapper_b200 import synth
 
 
-def dsm(rows, cols, res, n, reps):
+def dsm_setup(rows, cols, res, n):
+    """bench.py's dsm_c2-style cloud seeded in HBM, a device-resident map and a Dsm: (xyz, gm, dsm)."""
     dev = torch.device("cuda:0")
     g = torch.Generator(device=dev); g.manual_seed(2)
     half_x, half_y = rows * res / 2, cols * res / 2
@@ -20,7 +21,11 @@ def dsm(rows, cols, res, n, reps):
     torch.cuda.synchronize()
     gm = amb.AerialGridMap(amb.GridMapSettings(0, 0, rows * res, cols * res, res)).getMutable()
     gm.to_device(0, names=())
-    d = amb.Dsm(amb.DsmSettings(), gm)
+    return xyz, gm, amb.Dsm(amb.DsmSettings(), gm)
+
+
+def dsm(rows, cols, res, n, reps):
+    xyz, gm, d = dsm_setup(rows, cols, res, n)
     for r in range(reps):
         d.process_device(xyz.data_ptr(), n, gm)
         gm.sync()
