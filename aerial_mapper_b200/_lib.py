@@ -99,6 +99,7 @@ SYMBOLS = {
     "amb_dsm_process_sharded": (C.c_int, [_P, _P, _P, C.c_size_t, C.c_int32, C.c_double, C.c_double, C.c_uint32]),
     "amb_dsm_enable_debug": (C.c_int, [_P, C.c_int]),
     "amb_dsm_download_debug": (C.c_int, [_P, _P, _P]),
+    "amb_dsm_download_bins": (C.c_int, [_P, _P, _P, _P, _P]),
     "amb_dsm_thresholds": (C.c_int, [C.c_int32, _P, C.c_int32]),
     "amb_ortho_from_pcl_process": (C.c_int, [_P, _P, _P, C.c_size_t, C.c_int32, C.c_int32]),
     "amb_ortho_from_pcl_process_device": (C.c_int, [_P, _P, _P, C.c_size_t, C.c_int32, C.c_int32]),

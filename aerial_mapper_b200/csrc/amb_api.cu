@@ -5,6 +5,7 @@
 #include <new>
 
 #include "amb_context.h"
+#include "dsm_plan.h"
 
 namespace amb {
 
@@ -542,6 +543,37 @@ int amb_dsm_download_debug(amb_ctx* ctx, int32_t* neighbour_count, int8_t* thres
                                   cudaMemcpyDeviceToHost, ctx->stream));
   if (threshold_index)
     AMB_CUDA(ctx, cudaMemcpyAsync(threshold_index, ctx->dbg_level.ptr, cells, cudaMemcpyDeviceToHost, ctx->stream));
+  AMB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return AMB_OK;
+}
+
+int amb_dsm_download_bins(amb_ctx* ctx, int32_t* layout, uint32_t* bucket_starts, double* records, uint32_t* order) {
+  if (!ctx) return AMB_ERR_INVALID_ARGUMENT;
+  if (ctx->last_bin_destinations <= 0 || ctx->last_dsm_plan.size() != sizeof(dsmk::DsmPlan))
+    return AMB_ERR_INVALID_ARGUMENT;
+  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
+  dsmk::DsmPlan plan;
+  std::memcpy(&plan, ctx->last_dsm_plan.data(), sizeof(plan));
+  unsigned int n_binned = 0;  // counted by the partition kernel, independently of the bucket starts
+  AMB_CUDA(ctx, cudaMemcpyAsync(&n_binned, ctx->counters.as<unsigned int>() + CTR_DSM_BINNED, sizeof(n_binned),
+                                cudaMemcpyDeviceToHost, ctx->stream));
+  AMB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  if (layout) {
+    const int32_t v[AMB_DSM_BINS_LAYOUT] = {plan.B,   plan.Pa,  plan.BR,      plan.BC,
+                                            plan.KR,  plan.KC,  plan.gj0,     plan.tile_j0,
+                                            static_cast<int32_t>(n_binned),   ctx->last_bin_destinations};
+    std::memcpy(layout, v, sizeof(v));
+  }
+  const size_t nbk = static_cast<size_t>(plan.KR) * static_cast<size_t>(plan.KC);
+  if (bucket_starts)
+    AMB_CUDA(ctx, cudaMemcpyAsync(bucket_starts, ctx->bin_starts.ptr, (nbk + 1) * sizeof(uint32_t),
+                                  cudaMemcpyDeviceToHost, ctx->stream));
+  if (records && n_binned)
+    AMB_CUDA(ctx, cudaMemcpyAsync(records, ctx->records.ptr, static_cast<size_t>(n_binned) * sizeof(dsmk::PointRec),
+                                  cudaMemcpyDeviceToHost, ctx->stream));
+  if (order && n_binned)
+    AMB_CUDA(ctx, cudaMemcpyAsync(order, ctx->point_order.ptr, static_cast<size_t>(n_binned) * sizeof(uint32_t),
+                                  cudaMemcpyDeviceToHost, ctx->stream));
   AMB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return AMB_OK;
 }

@@ -200,6 +200,7 @@ struct amb_ctx {
   int64_t last_points_binned = 0, last_cells_empty = 0;
   std::vector<unsigned char> last_dsm_plan;  // the DsmPlan of the last dsm_run (read by the adaptive OrthoFromPcl pass;
                                              // on a stripe: of its whole-map binning, dsm_run(.., whole_map_bins))
+  int32_t last_bin_destinations = 0;         // coarse destinations S of the last binning (0: none yet; amb_dsm_download_bins)
 
   // Ortho scratch
   amb::DeviceBuffer frames;       // device copies of the caller's frames (host entry point)

@@ -830,6 +830,9 @@ int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, 
   unsigned int* counters = ctx->counters.as<unsigned int>();
   PointRec* rec = ctx->records.as<PointRec>();
 
+  // the bins are rewritten from here on: until this call stores its plan they describe no plan
+  ctx->last_dsm_plan.clear();
+  ctx->last_bin_destinations = 0;
   AMB_CUDA(ctx, cudaMemsetAsync(G, 0, g_elems * sizeof(unsigned int), s));
   AMB_CUDA(ctx, cudaMemsetAsync(ctx->bucket_flags.ptr, 0, nbk, s));
   // only this stage's own slots: the sticky CHECK flags of earlier asynchronous calls stay until they are reported
@@ -907,6 +910,7 @@ int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, 
                                                 ctx->block_sums.as<unsigned int>());
   dsm_fine_scatter_kernel<<<static_cast<unsigned int>(pp.S) * pp.n_groups, kFineThreads, 0, s>>>(
       plan, pp, ctx->records_tmp.as<PointRec>(), ctx->tile_offsets.as<unsigned short>(), G, rec);
+  ctx->last_bin_destinations = pp.S;
   // Canonical order inside the buckets: Dsm orders only the buckets its warp-per-cell kernel will read (marked from the
   // cell list after the gather); OrthoFromPcl's adaptive pass may read any bucket, so that mode orders all of them here.
   unsigned char* bucket_flags = ctx->bucket_flags.as<unsigned char>();

@@ -260,6 +260,19 @@ int amb_dsm_process_sharded(amb_ctx* ctx, const double* xyz, const uint64_t* ids
  * produced them (0 = first query succeeded, 1.. = expanding-radius retries dsm.cc:133-144, -1 = cell untouched). */
 int amb_dsm_enable_debug(amb_ctx* ctx, int enable);
 int amb_dsm_download_debug(amb_ctx* ctx, int32_t* neighbour_count, int8_t* threshold_index);
+/* The bins of the last binning on this context (Dsm, OrthoFromPcl, or the whole-map re-binning of an adaptive
+ * OrthoFromPcl stripe), for tests of the binning stage.  Synchronises the context's stream; AMB_ERR_INVALID_ARGUMENT
+ * before the first binning.  Every buffer may be NULL: a first call with NULL buffers but `layout` returns the sizes.
+ *   layout         AMB_DSM_BINS_LAYOUT int32: B, Pa, BR, BC, KR, KC, gj0, tile_j0 (the plan's bin grid), n_binned, and
+ *                  S, the number of coarse destinations the partition used
+ *   bucket_starts  KR*KC + 1 uint32: record range [G[b], G[b + 1]) of bucket b = (bi >> log2 B) + (bj >> log2 B) * KR
+ *   records        4 * n_binned doubles, bit for bit: x - center_northing, y - center_easting, z (OrthoFromPcl:
+ *                  double(intensity)), and a word whose low 32 bits are the point's id (array position or caller id)
+ *                  and high 32 bits (bi << 4) | (bj & 15)
+ *   order          n_binned uint32: per bucket, its record positions by ascending id.  OrthoFromPcl orders every bucket;
+ *                  Dsm only the buckets its warp-per-cell pass reads (the other entries are unspecified). */
+#define AMB_DSM_BINS_LAYOUT 10
+int amb_dsm_download_bins(amb_ctx* ctx, int32_t* layout, uint32_t* bucket_starts, double* records, uint32_t* order);
 /* The thresholds lambda_k * radius the reference's retry loop visits (dsm.cc:133-144), computed with its exact
  * recurrence.  Returns the count (<= capacity) or a negative status. */
 int amb_dsm_thresholds(int32_t interpolation_radius, double* thresholds, int32_t capacity);

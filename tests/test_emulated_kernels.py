@@ -39,7 +39,8 @@ def test_variant_gpu_tests_pass_on_the_emulated_kernels(sched):
     # also with the block's threads scheduled in reverse and in a fresh pseudo-random order every round: a kernel whose
     # result depended on who runs first (e.g. a missing barrier between a write and another thread's read) would differ
     tail = run_child("gpu", ["test_gpu_ortho_dominance.py", "test_gpu_compact_mirrors.py", "test_ortho_from_pcl.py",
-                             "test_stereo_rectify.py", "test_gpu_dsm_adversarial.py", "test_gpu_dsm_heights.py"], sched=sched)
+                             "test_stereo_rectify.py", "test_gpu_dsm_adversarial.py", "test_gpu_dsm_heights.py",
+                             "test_gpu_dsm_binning.py"], sched=sched)
     assert " passed" in tail and "failed" not in tail
 
 
