@@ -135,7 +135,8 @@ extern "C" int amb_stereo_reproject_device(int device, void* stream, const float
                                            int32_t* d_out_intensity, size_t capacity, uint32_t* d_block_scratch,
                                            unsigned long long* d_count) {
   if (!d_disparity || !d_image_left || !K || !R_G_C || !t_G_C1 || !d_out_xyz || !d_out_intensity || !d_block_scratch ||
-      !d_count || width <= 0 || height <= 0)
+      !d_count || width <= 0 || height <= 0 || disparity_stride < static_cast<size_t>(width) ||
+      image_stride < static_cast<size_t>(width))
     return AMB_ERR_INVALID_ARGUMENT;
   if (baseline == 0.0) return AMB_ERR_CHECK_FAILED;  // CHECK_NE(baseline, 0.0), densifier.cpp:39
   if (cudaSetDevice(device) != cudaSuccess) {
@@ -173,7 +174,8 @@ extern "C" int amb_stereo_reproject(int device, const float* disparity, size_t d
                                     const double* K, double baseline, const double* R_G_C, const double* t_G_C1,
                                     float max_invalid_disparity, double* out_xyz, int32_t* out_intensity,
                                     size_t capacity, size_t* out_count) {
-  if (!disparity || !image_left || !out_xyz || !out_intensity || !out_count || width <= 0 || height <= 0)
+  if (!disparity || !image_left || !out_xyz || !out_intensity || !out_count || width <= 0 || height <= 0 ||
+      disparity_stride < static_cast<size_t>(width) || image_stride < static_cast<size_t>(width))
     return AMB_ERR_INVALID_ARGUMENT;
   int n_dev = 0;
   if (cudaGetDeviceCount(&n_dev) != cudaSuccess || n_dev <= 0) {

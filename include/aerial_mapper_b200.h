@@ -326,7 +326,8 @@ int amb_ortho_from_pcl_process_sharded(amb_ctx* ctx, const double* xyz, const in
  * P = R_G_C p + t_G_C1; kept unless (float)P.z is infinite.  Kept points (double[3]) and their gray values are
  * written in raster order (point_cloud_eigen / point_cloud_intensities).  K = {fx, fy, cx, cy}; R_G_C row-major.
  * *out_count = number of valid points (may exceed capacity: only the first `capacity` were written).
- * Strides are in elements (floats / bytes) per row. */
+ * Strides are in elements (floats / bytes) per row and at least `width`; a smaller stride, a NULL pointer or a
+ * width or height <= 0 returns AMB_ERR_INVALID_ARGUMENT, a zero baseline AMB_ERR_CHECK_FAILED. */
 int amb_stereo_reproject(int device, const float* disparity, size_t disparity_stride, const uint8_t* image_left,
                          size_t image_stride, int32_t width, int32_t height, const double* K, double baseline,
                          const double* R_G_C, const double* t_G_C1, float max_invalid_disparity, double* out_xyz,

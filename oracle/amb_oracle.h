@@ -83,7 +83,8 @@ int ambo_ortho_process(const amb_geometry* geom, const float* elevation, float* 
                        int64_t cell_end, double* seconds);
 
 /* stereo::Densifier::computePointCloud restated (densifier.cpp:25-108; "next" row N3): disparity -> world points in
- * raster order.  K = {fx, fy, cx, cy}; strides in elements per row. */
+ * raster order.  K = {fx, fy, cx, cy}; strides in elements per row, at least `width` (the product's argument
+ * contract, include/aerial_mapper_b200.h). */
 int ambo_stereo_reproject(const float* disparity, size_t disparity_stride, const uint8_t* image_left,
                           size_t image_stride, int32_t width, int32_t height, const double* K, double baseline,
                           const double* R_G_C, const double* t_G_C1, float max_invalid_disparity, double* out_xyz,

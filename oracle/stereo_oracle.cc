@@ -15,7 +15,8 @@ extern "C" int ambo_stereo_reproject(const float* disparity, size_t disparity_st
                                      double baseline, const double* R_G_C, const double* t_G_C1,
                                      float max_invalid_disparity, double* out_xyz, int32_t* out_intensity,
                                      size_t capacity, size_t* out_count) {
-  if (!disparity || !image_left || !K || !R_G_C || !t_G_C1 || !out_xyz || !out_intensity || !out_count)
+  if (!disparity || !image_left || !K || !R_G_C || !t_G_C1 || !out_xyz || !out_intensity || !out_count || width <= 0 ||
+      height <= 0 || disparity_stride < static_cast<size_t>(width) || image_stride < static_cast<size_t>(width))
     return AMB_ERR_INVALID_ARGUMENT;
   if (baseline == 0.0) return AMB_ERR_CHECK_FAILED; /* CHECK_NE(baseline, 0.0), :39 */
   const double fx = K[0], fy = K[1], cx = K[2], cy = K[3];

@@ -40,7 +40,7 @@ def test_variant_gpu_tests_pass_on_the_emulated_kernels(sched):
     # result depended on who runs first (e.g. a missing barrier between a write and another thread's read) would differ
     tail = run_child("gpu", ["test_gpu_ortho_dominance.py", "test_gpu_compact_mirrors.py", "test_ortho_from_pcl.py",
                              "test_stereo_rectify.py", "test_gpu_dsm_adversarial.py", "test_gpu_dsm_heights.py",
-                             "test_gpu_dsm_binning.py"], sched=sched)
+                             "test_gpu_dsm_binning.py", "test_gpu_stereo_device.py"], sched=sched)
     assert " passed" in tail and "failed" not in tail
 
 
