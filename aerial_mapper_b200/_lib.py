@@ -29,6 +29,10 @@ LAYER_ID = {name: k for k, name in enumerate(LAYER_NAMES)}
 
 DIST_NONE, DIST_RADTAN, DIST_EQUIDISTANT, DIST_FOV = 0, 1, 2, 3
 DSM_F64, DSM_F32 = 0, 1
+# amb_raster_format: pixel formats of amb_export_raster, and their bytes per pixel
+RASTER_F32, RASTER_GRAY8, RASTER_BGR8, RASTER_MASK8 = 0, 1, 2, 3
+RASTER_FORMAT = {"f32": RASTER_F32, "gray8": RASTER_GRAY8, "bgr8": RASTER_BGR8, "mask8": RASTER_MASK8}
+RASTER_BPP = {RASTER_F32: 4, RASTER_GRAY8: 1, RASTER_BGR8: 3, RASTER_MASK8: 1}
 
 
 class Geometry(C.Structure):
@@ -134,6 +138,10 @@ SYMBOLS = {
     "amb_multi_dsm_process": (C.c_int, [_P, _P, C.c_size_t, C.c_int32, C.c_double, C.c_double]),
     "amb_multi_ortho_process": (C.c_int, [_P, C.POINTER(Camera), _P, _P, C.c_size_t, C.c_int32, C.c_size_t, C.c_int32]),
     "amb_multi_ortho_from_pcl_process": (C.c_int, [_P, _P, _P, C.c_size_t, C.c_int32, C.c_int32]),
+    "amb_raster_geotransform": (C.c_int, [C.POINTER(Geometry), C.POINTER(C.c_double)]),
+    "amb_export_raster": (C.c_int, [_P, C.c_int, C.c_int, _P]),
+    "amb_export_raster_device": (C.c_int, [_P, C.c_int, C.c_int, _P]),
+    "amb_multi_export_raster": (C.c_int, [_P, C.c_int, C.c_int, _P]),
     "amb_get_timings": (C.c_int, [_P, C.POINTER(Timings)]),
     "amb_host_alloc": (C.c_int, [C.POINTER(_P), C.c_size_t]),
     "amb_host_free": (C.c_int, [_P]),

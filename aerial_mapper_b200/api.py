@@ -185,6 +185,36 @@ class GridMap(object):
         if self._ctx is not None:
             check(lib().amb_sync(self._ctx), self._ctx)
 
+    # --- north-up raster export (convention: include/aerial_mapper_b200.h, amb_raster_format) ---
+    def geotransform(self):
+        """GDAL geotransform of the exported raster: (west, res, 0, north, 0, -res)."""
+        gt = (C.c_double * 6)()
+        check(lib().amb_raster_geotransform(C.byref(self.geometry), gt))
+        return tuple(gt)
+
+    def to_raster(self, name, fmt="f32", out=None):
+        """The context's band of layer `name` as a north-up, row-major raster converted on the device: float32 or uint8
+        [band_rows, rows], or uint8 [band_rows, rows, 3] (B, G, R) for "bgr8"; band_rows = col_end - col_begin, and image
+        row r of the whole map is layer column r read backwards.  fmt: "f32", "gray8", "bgr8" or "mask8".  `out`: an
+        optional C-contiguous array of that shape and dtype to write into (e.g. the context's rows of a full image, or
+        page-locked memory)."""
+        if not self._resident:
+            raise AmbError(_lib.AMB_ERR_INVALID_ARGUMENT,
+                           "to_raster exports device-resident layers: call to_device() first")
+        f = _lib.RASTER_FORMAT[fmt] if isinstance(fmt, str) else int(fmt)
+        if f not in _lib.RASTER_BPP:
+            raise AmbError(_lib.AMB_ERR_INVALID_ARGUMENT, "raster format %r" % (fmt,))
+        c0, c1 = self._col_range
+        shape = (c1 - c0, self.geometry.rows) + ((3,) if f == _lib.RASTER_BGR8 else ())
+        dtype = np.float32 if f == _lib.RASTER_F32 else np.uint8
+        if out is None:
+            out = np.empty(shape, dtype)
+        elif out.shape != shape or out.dtype != dtype or not out.flags.c_contiguous:
+            raise AmbError(_lib.AMB_ERR_SIZE_MISMATCH, "out must be C-contiguous %s %r" % (np.dtype(dtype).name, shape))
+        ctx = self._ctx
+        check(lib().amb_export_raster(ctx, LAYER_ID[name], f, out.ctypes.data_as(C.c_void_p)), ctx)
+        return out
+
     def timings(self):
         t = _lib.Timings()
         check(lib().amb_get_timings(self.context(), C.byref(t)), self._ctx)

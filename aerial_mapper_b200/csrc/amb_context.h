@@ -183,6 +183,7 @@ struct amb_ctx {
   amb::DeviceBuffer counters;     // small flag/counter block, see amb::CounterSlot
   amb::DeviceBuffer dbg_count;    // int32 per slab cell
   amb::DeviceBuffer dbg_level;    // int8 per slab cell
+  amb::DeviceBuffer raster_band;  // amb_export_raster: the converted band before its copy to the host
   double dsm_density_hint = 0.0;  // points per cell of the whole cloud (0: derive from the points passed)
   bool dsm_debug = false;
   int dsm_stream_chunks = 4;  // (> 1, only with a host mirror of the output layer) gather + fill in column chunks, each chunk's

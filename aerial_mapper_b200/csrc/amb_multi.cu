@@ -119,6 +119,18 @@ int amb_multi_download_layer(amb_multi* m, int layer, float* host_full) {
   return for_each_stripe(m, [&](int r, amb_ctx* c) { return amb_download_layer(c, layer, stripe_ptr(m, r, host_full)); });
 }
 
+int amb_multi_export_raster(amb_multi* m, int layer, int format, void* host_image) {
+  if (!m || !host_image || layer < 0 || layer >= AMB_NUM_LAYERS || format < AMB_RASTER_F32 || format > AMB_RASTER_MASK8)
+    return AMB_ERR_INVALID_ARGUMENT;
+  const size_t bpp = format == AMB_RASTER_F32 ? 4 : format == AMB_RASTER_BGR8 ? 3 : 1;
+  // stripe r owns image rows [col_begin, col_end) (include/aerial_mapper_b200.h)
+  return for_each_stripe(m, [&](int, amb_ctx* c) {
+    unsigned char* band = static_cast<unsigned char*>(host_image) +
+                          static_cast<size_t>(m->geom.rows) * static_cast<size_t>(c->col_begin) * bpp;
+    return amb_export_raster(c, layer, format, band);
+  });
+}
+
 int amb_multi_set_host_mirror(amb_multi* m, int layer, float* host_full) {
   if (!m) return AMB_ERR_INVALID_ARGUMENT;
   for (size_t r = 0; r < m->ctx.size(); ++r) {

@@ -415,6 +415,42 @@ int amb_multi_ortho_process(amb_multi* m, const amb_camera* camera, const double
 int amb_multi_ortho_from_pcl_process(amb_multi* m, const double* xyz, const int32_t* intensities, size_t n,
                                      int32_t interpolation_radius, int32_t use_adaptive_interpolation);
 
+/* ---- export of a layer as a north-up georeferenced raster ("next" row N4) ----
+ * Convention.  A map of rows x cols cells (rows = size(0) along x / easting, cols = size(1) along y / northing, cell
+ * (0,0) at the max-x / max-y corner) is exported as an image W = rows pixels wide and H = cols pixels high, row-major,
+ * north-up and east-right:
+ *     pixel (r, c) = layer(i = rows - 1 - c, j = r)        r in [0, cols), c in [0, rows)
+ * Image row r is layer column r read backwards: a per-column reversal plus a value conversion, no transpose.  A context
+ * owning columns [col_begin, col_end) owns exactly image rows [col_begin, col_end), so stripes write disjoint, contiguous
+ * bands of one image.  Geotransform in GDAL order (amb_raster_geotransform):
+ *     gt = { pos_x - length_x/2, res, 0, pos_y + length_y/2, 0, -res }
+ * The centre of pixel (r, c), (gt[0] + (c + 0.5) res, gt[3] - (r + 0.5) res), is amb_geometry_position(rows-1-c, r) up to
+ * rounding.  Pixel formats (bytes per pixel):
+ *   AMB_RASTER_F32    4  the layer's float32 bits, exactly (NaN payloads included: a DEM with NaN as no-data)
+ *   AMB_RASTER_GRAY8  1  OpenCV saturate_cast<uchar>(float): round half to even, clamp to [0, 255]; NaN, +inf and every
+ *                        value at or above 2^31 give 0 (cvRound's out-of-range result is INT_MIN, which saturates to 0)
+ *   AMB_RASTER_BGR8   3  colored_ortho's packed 0x00RRGGBB bits as the bytes B, G, R (CV_8UC3 order), top byte ignored,
+ *                        NaN -> 0, 0, 0; read as bits only, packed colours are float denormals
+ *   AMB_RASTER_MASK8  1  0 where the layer is NaN (any payload), 255 elsewhere
+ * `host_band` / `device_band` point at image row col_begin (the caller offsets a full-image pointer by
+ * col_begin * rows * bytes-per-pixel, the slab convention of amb_upload_layer); exactly (col_end - col_begin) * rows *
+ * bytes-per-pixel bytes are written, rows packed, at any byte alignment.  A NULL pointer, a bad layer or a bad format
+ * returns AMB_ERR_INVALID_ARGUMENT and writes nothing. */
+typedef enum amb_raster_format {
+  AMB_RASTER_F32 = 0,
+  AMB_RASTER_GRAY8 = 1,
+  AMB_RASTER_BGR8 = 2,
+  AMB_RASTER_MASK8 = 3
+} amb_raster_format;
+/* Host arithmetic, no GPU. */
+int amb_raster_geotransform(const amb_geometry* geom, double gt[6]);
+/* Synchronous: converted in HBM, then copied like amb_download_layer (pinned or pageable destination). */
+int amb_export_raster(amb_ctx* ctx, int layer, int format, void* host_band);
+/* Asynchronous on the context's stream, into device memory valid on the context's device. */
+int amb_export_raster_device(amb_ctx* ctx, int layer, int format, void* device_band);
+/* Every stripe of amb_multi writes its band of the caller's full image (rows x cols pixels), all devices at once. */
+int amb_multi_export_raster(amb_multi* m, int layer, int format, void* host_image);
+
 /* ---- measurement ---- */
 int amb_get_timings(amb_ctx* ctx, amb_timings* out);
 
