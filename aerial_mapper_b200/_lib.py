@@ -33,6 +33,8 @@ DSM_F64, DSM_F32 = 0, 1
 RASTER_F32, RASTER_GRAY8, RASTER_BGR8, RASTER_MASK8 = 0, 1, 2, 3
 RASTER_FORMAT = {"f32": RASTER_F32, "gray8": RASTER_GRAY8, "bgr8": RASTER_BGR8, "mask8": RASTER_MASK8}
 RASTER_BPP = {RASTER_F32: 4, RASTER_GRAY8: 1, RASTER_BGR8: 3, RASTER_MASK8: 1}
+# amb_resample: resampling of amb_import_raster
+RESAMPLE = {"nearest": 0, "bilinear": 1}
 
 
 class Geometry(C.Structure):
@@ -142,6 +144,14 @@ SYMBOLS = {
     "amb_export_raster": (C.c_int, [_P, C.c_int, C.c_int, _P]),
     "amb_export_raster_device": (C.c_int, [_P, C.c_int, C.c_int, _P]),
     "amb_multi_export_raster": (C.c_int, [_P, C.c_int, C.c_int, _P]),
+    "amb_import_raster": (C.c_int, [_P, C.c_int, _P, C.c_int32, C.c_int32, C.c_size_t, C.POINTER(C.c_double), C.c_int,
+                                    C.c_float, C.c_int]),
+    "amb_import_raster_device": (C.c_int, [_P, C.c_int, _P, C.c_int32, C.c_int32, C.c_size_t, C.POINTER(C.c_double),
+                                           C.c_int, C.c_float, C.c_int]),
+    "amb_multi_import_raster": (C.c_int, [_P, C.c_int, _P, C.c_int32, C.c_int32, C.c_size_t, C.POINTER(C.c_double),
+                                          C.c_int, C.c_float, C.c_int]),
+    "amb_raster_import_tables": (C.c_int, [C.POINTER(Geometry), C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                           C.POINTER(C.c_double), C.c_int, _P, _P, _P, _P]),
     "amb_get_timings": (C.c_int, [_P, C.POINTER(Timings)]),
     "amb_host_alloc": (C.c_int, [C.POINTER(_P), C.c_size_t]),
     "amb_host_free": (C.c_int, [_P]),

@@ -215,6 +215,27 @@ class GridMap(object):
         check(lib().amb_export_raster(ctx, LAYER_ID[name], f, out.ctypes.data_as(C.c_void_p)), ctx)
         return out
 
+    def from_raster(self, name, band, geotransform, nodata=None, resample="bilinear"):
+        """Resample a north-up float32 raster into the context's stripe of layer `name` on the device (convention:
+        include/aerial_mapper_b200.h, amb_resample): band is float32 [H, W] with unit element stride (a row-sliced view
+        is fine), geotransform its GDAL geotransform (west, res_x, 0, north, 0, -res_y) in the map's projected frame.
+        NaN pixels, and pixels equal to `nodata` if given, are no-data; cells outside the raster or fed by no-data keep
+        their value.  resample: "bilinear" or "nearest"; a raster on the map's own grid is copied bit for bit by both."""
+        if not self._resident:
+            raise AmbError(_lib.AMB_ERR_INVALID_ARGUMENT,
+                           "from_raster imports into device-resident layers: call to_device() first")
+        r = _lib.RESAMPLE[resample] if isinstance(resample, str) else int(resample)
+        a = np.asarray(band)
+        if a.ndim != 2 or a.dtype != np.float32 or a.strides[1] != 4 or a.strides[0] < 4 * a.shape[1]:
+            raise AmbError(_lib.AMB_ERR_INVALID_ARGUMENT,
+                           "band must be float32 [H, W] with unit element stride and increasing rows; got %s %r strides %r"
+                           % (a.dtype, a.shape, a.strides))
+        gt = (C.c_double * 6)(*[float(v) for v in geotransform])
+        ctx = self._ctx
+        check(lib().amb_import_raster(ctx, LAYER_ID[name], a.ctypes.data_as(C.c_void_p), a.shape[1], a.shape[0],
+                                      a.strides[0], gt, 0 if nodata is None else 1,
+                                      0.0 if nodata is None else float(nodata), r), ctx)
+
     def timings(self):
         t = _lib.Timings()
         check(lib().amb_get_timings(self.context(), C.byref(t)), self._ctx)

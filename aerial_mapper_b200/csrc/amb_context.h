@@ -183,7 +183,9 @@ struct amb_ctx {
   amb::DeviceBuffer counters;     // small flag/counter block, see amb::CounterSlot
   amb::DeviceBuffer dbg_count;    // int32 per slab cell
   amb::DeviceBuffer dbg_level;    // int8 per slab cell
-  amb::DeviceBuffer raster_band;  // amb_export_raster: the converted band before its copy to the host
+  amb::DeviceBuffer raster_band;  // amb_export_raster: the converted band before its copy to the host;
+                                  // amb_import_raster: the raster window after its copy to the device
+  amb::DeviceBuffer raster_taps;  // amb_import_raster*: the per-axis tables of the last import
   double dsm_density_hint = 0.0;  // points per cell of the whole cloud (0: derive from the points passed)
   bool dsm_debug = false;
   int dsm_stream_chunks = 4;  // (> 1, only with a host mirror of the output layer) gather + fill in column chunks, each chunk's

@@ -131,6 +131,15 @@ int amb_multi_export_raster(amb_multi* m, int layer, int format, void* host_imag
   });
 }
 
+int amb_multi_import_raster(amb_multi* m, int layer, const float* host_band, int32_t width, int32_t height,
+                            size_t row_stride, const double gt[6], int has_nodata, float nodata, int resample) {
+  if (!m) return AMB_ERR_INVALID_ARGUMENT;
+  // every stripe validates the same arguments before it writes anything, and reads only its own window of the band
+  return for_each_stripe(m, [&](int, amb_ctx* c) {
+    return amb_import_raster(c, layer, host_band, width, height, row_stride, gt, has_nodata, nodata, resample);
+  });
+}
+
 int amb_multi_set_host_mirror(amb_multi* m, int layer, float* host_full) {
   if (!m) return AMB_ERR_INVALID_ARGUMENT;
   for (size_t r = 0; r < m->ctx.size(); ++r) {

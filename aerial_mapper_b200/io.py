@@ -9,8 +9,12 @@
 and the output side ("next" row N4):
 
     write_geotiff                   :349-509   toGeoTiff / writeDataToDEMGeoTiffColor, with the map's geotransform
+
+and back in: read_geotiff, the DEM GeoTIFFs GDAL writes (GridMap.from_raster resamples them into a layer).
 """
+import math
 import struct
+import zlib
 
 import numpy as np
 
@@ -226,3 +230,158 @@ def write_geotiff(path, raster, geotransform, epsg=32632, nodata=None):
             if bands == 3:
                 part = part[:, :, ::-1]               # B, G, R -> R, G, B, this strip only
             f.write(np.ascontiguousarray(part, dtype=a.dtype.newbyteorder("<")).tobytes())
+
+
+# ---- GeoTIFF reader: the subset GDAL writes for DEMs ----
+_TIFF_TYPES = {1: "B", 2: "s", 3: "H", 4: "I", 5: "II", 6: "b", 7: "B", 8: "h", 9: "i", 10: "ii", 11: "f", 12: "d"}
+_SAMPLE_DTYPES = {(8, 1): np.uint8, (16, 2): np.int16, (16, 1): np.uint16, (32, 2): np.int32, (32, 3): np.float32,
+                  (64, 3): np.float64}
+
+
+def _unsupported(tag, value, why):
+    raise ValueError("read_geotiff: %s = %r is not supported (%s)" % (tag, value, why))
+
+
+def _read_ifd(data):
+    """Tag -> tuple of values (ASCII: str) of the first IFD of a classic little-endian TIFF."""
+    if len(data) < 8:
+        raise ValueError("read_geotiff: not a TIFF file (%d bytes)" % len(data))
+    if data[:2] == b"MM":
+        _unsupported("byte order", "MM", "big-endian TIFF")
+    if data[:2] != b"II":
+        raise ValueError("read_geotiff: not a TIFF file (byte order mark %r)" % data[:2])
+    magic = struct.unpack_from("<H", data, 2)[0]
+    if magic == 43:
+        _unsupported("version", 43, "BigTIFF")
+    if magic != 42:
+        raise ValueError("read_geotiff: not a TIFF file (version %d)" % magic)
+    at = struct.unpack_from("<I", data, 4)[0]
+    n = struct.unpack_from("<H", data, at)[0]
+    tags = {}
+    for e in range(n):
+        tag, typ, count, raw = struct.unpack_from("<HHI4s", data, at + 2 + 12 * e)
+        if typ not in _TIFF_TYPES:
+            _unsupported("type of tag %d" % tag, typ, "not a classic TIFF field type")
+        fmt = _TIFF_TYPES[typ]
+        size = struct.calcsize("<" + fmt) * count
+        buf = raw if size <= 4 else data[struct.unpack("<I", raw)[0]:struct.unpack("<I", raw)[0] + size]
+        if typ == 2:
+            tags[tag] = buf[:count].split(b"\0")[0].decode("ascii", "replace")
+        else:
+            tags[tag] = struct.unpack_from("<%d%s" % (count * len(fmt), fmt[0]), buf)
+    return tags
+
+
+def _geotransform(tags):
+    if 34264 in tags:                                   # ModelTransformation, row-major 4 x 4
+        m = tags[34264]
+        if len(m) != 16:
+            _unsupported("ModelTransformation", m, "16 values expected")
+        if m[1] != 0.0 or m[4] != 0.0:
+            _unsupported("ModelTransformation", m, "rotated geotransform")
+        gt = [m[3], m[0], m[1], m[7], m[4], m[5]]
+    elif 33550 in tags and 33922 in tags:               # ModelPixelScale + ModelTiepoint (I, J, K, X, Y, Z)
+        sx, sy = tags[33550][0], tags[33550][1]
+        tp = tags[33922]
+        if len(tp) != 6:
+            _unsupported("ModelTiepoint", tp, "exactly one tiepoint expected")
+        i, j, x, y = tp[0], tp[1], tp[3], tp[4]
+        gt = [x - i * sx, sx, 0.0, y + j * sy, 0.0, -sy]
+    else:
+        raise ValueError("read_geotiff: no georeferencing (ModelPixelScale + ModelTiepoint or ModelTransformation)")
+    keys = _geokeys(tags)
+    if keys.get(1025) == 2:                             # GTRasterTypeGeoKey = RasterPixelIsPoint: GDAL's half-pixel shift
+        gt[0] -= 0.5 * gt[1] + 0.5 * gt[2]
+        gt[3] -= 0.5 * gt[4] + 0.5 * gt[5]
+    if not all(math.isfinite(v) for v in gt) or not gt[1] > 0.0 or not gt[5] < 0.0:
+        _unsupported("geotransform", tuple(gt), "north-up (x0, res, 0, y0, 0, -res) only")
+    return tuple(float(v) for v in gt)
+
+
+def _geokeys(tags):
+    """GeoKeyDirectory: key id -> SHORT value stored in the directory itself (the keys read here are all such)."""
+    d = tags.get(34735, ())
+    keys = {}
+    for k in range(1, (len(d) // 4)):
+        kid, loc, count, val = d[4 * k:4 * k + 4]
+        if loc == 0 and count == 1:
+            keys[kid] = val
+    return keys
+
+
+def _undo_predictor(chunk, predictor, dtype, rows, cols, spp):
+    """chunk: the decoded bytes of `rows` rows of `cols` pixels of `spp` samples -> dtype [rows, cols, spp]."""
+    item = np.dtype(dtype).itemsize
+    raw = np.frombuffer(chunk, np.uint8, rows * cols * spp * item)
+    if predictor == 3:                                  # byte planes, most significant first, differenced with stride spp
+        b = raw.reshape(rows, cols, spp * item)
+        b = np.cumsum(b.reshape(rows, cols * item, spp), axis=1, dtype=np.uint8).reshape(rows, item, cols * spp)
+        be = np.ascontiguousarray(b.transpose(0, 2, 1))  # [rows, samples, bytes MSB..LSB]
+        return be.view(np.dtype(dtype).newbyteorder(">")).reshape(rows, cols, spp).astype(dtype)
+    a = raw.view(np.dtype(dtype).newbyteorder("<")).reshape(rows, cols, spp).astype(dtype)
+    if predictor == 2:                                  # horizontal differencing, modulo the sample type
+        a = np.cumsum(a, axis=1, dtype=dtype)
+    return a
+
+
+def read_geotiff(path, band=0):
+    """A band of a GeoTIFF as GDAL writes DEMs: (array [H, W] in the file's sample type, GDAL geotransform (west, res_x, 0,
+    north, 0, -res_y), EPSG code or None, no-data value or None).
+
+    Reads classic little-endian TIFF (first IFD, PlanarConfiguration 1), strips or tiles, uncompressed or Deflate,
+    predictor 1, 2 (integer samples) or 3 (floating point), samples uint8, int16, uint16, int32, float32 or float64.  The
+    geotransform comes from ModelPixelScale + ModelTiepoint (one tiepoint, at any raster point) or from a
+    ModelTransformation without rotation; GTRasterTypeGeoKey = PixelIsPoint shifts it by half a pixel, as GDAL reads it.
+    EPSG: ProjectedCSTypeGeoKey, else GeographicTypeGeoKey.  No-data: GDAL_NODATA as a float ("nan" included).  Anything
+    else raises ValueError naming the tag and value (BigTIFF, big-endian, LZW, JPEG, rotated transforms ...).
+
+    For GridMap.from_raster a DEM is converted with a.astype(np.float32), its no-data value passed along: that value must
+    be exact in float32 (true of every int16 and uint16 value) or pixels holding it will not compare equal."""
+    with open(path, "rb") as f:
+        data = f.read()
+    tags = _read_ifd(data)
+    width, height = tags[256][0], tags[257][0]
+    spp = tags.get(277, (1,))[0]
+    planar = tags.get(284, (1,))[0]
+    if planar != 1:
+        _unsupported("PlanarConfiguration", planar, "chunky (1) only")
+    bits = set(tags.get(258, (1,)))
+    fmt = set(tags.get(339, (1,)))
+    if len(bits) != 1 or len(fmt) != 1 or (bits.pop(), fmt.pop()) not in _SAMPLE_DTYPES:
+        _unsupported("BitsPerSample / SampleFormat", (tags.get(258), tags.get(339)),
+                     "uint8, int16, uint16, int32, float32 or float64 samples")
+    dtype = _SAMPLE_DTYPES[(tags[258][0], tags.get(339, (1,))[0])]
+    if not 0 <= band < spp:
+        raise ValueError("read_geotiff: band %d of %d" % (band, spp))
+    comp = tags.get(259, (1,))[0]
+    if comp not in (1, 8, 32946):
+        _unsupported("Compression", comp, "none (1) or Deflate (8, 32946) only")
+    predictor = tags.get(317, (1,))[0]
+    is_float = np.dtype(dtype).kind == "f"
+    if predictor not in (1, 2, 3) or (predictor == 2 and is_float) or (predictor == 3 and not is_float):
+        _unsupported("Predictor", predictor, "1, 2 for integer or 3 for floating-point samples")
+    if 322 in tags:                                     # tiles
+        tw, th = tags[322][0], tags[323][0]
+        offsets, counts = tags[324], tags[325]
+        across = (width + tw - 1) // tw
+        grid = [((k // across) * th, (k % across) * tw, th, tw) for k in range(len(offsets))]
+    elif 273 in tags:                                   # strips
+        rps = min(tags.get(278, (height,))[0], height)
+        offsets, counts = tags[273], tags[279]
+        grid = [(k * rps, 0, min(rps, height - k * rps), width) for k in range(len(offsets))]
+    else:
+        raise ValueError("read_geotiff: neither strips nor tiles")
+    out = np.empty((height, width), dtype)
+    for (r0, c0, rows, cols), at, n in zip(grid, offsets, counts):
+        if r0 >= height or c0 >= width:
+            continue
+        chunk = data[at:at + n]
+        if comp != 1:
+            chunk = zlib.decompress(chunk)
+        a = _undo_predictor(chunk, predictor, dtype, rows, cols, spp)
+        out[r0:r0 + rows, c0:c0 + cols] = a[:height - r0, :width - c0, band]
+    keys = _geokeys(tags)
+    epsg = keys.get(3072, keys.get(2048))
+    nodata = tags.get(42113)
+    return out, _geotransform(tags), (None if epsg in (None, 0, 32767) else int(epsg)), \
+        (None if nodata is None else float(nodata.strip()))

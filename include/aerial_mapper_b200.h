@@ -451,6 +451,47 @@ int amb_export_raster_device(amb_ctx* ctx, int layer, int format, void* device_b
 /* Every stripe of amb_multi writes its band of the caller's full image (rows x cols pixels), all devices at once. */
 int amb_multi_export_raster(amb_multi* m, int layer, int format, void* host_image);
 
+/* ---- import of a north-up raster into a layer, resampled to the map grid ----
+ * Source.  A float32 band of width x height pixels, row-major, rows `row_stride` bytes apart (a multiple of 4, at least
+ * 4 * width), with a GDAL-order geotransform gt[6] that is north-up (gt[2] == gt[4] == 0, gt[1] > 0, gt[5] < 0, all
+ * finite): pixel (r, c) covers [gt0 + c gt1, gt0 + (c+1) gt1) x (gt3 + (r+1) gt5, gt3 + r gt5] (PixelIsArea, as
+ * amb_raster_geotransform).  NaN is always no-data; with has_nodata, pixels that compare equal to `nodata` are no-data
+ * too (IEEE equality: nodata 0 also matches -0).  The raster is in the map's planar frame (x = easting, y = northing,
+ * the same projected CRS); nothing is reprojected.
+ * Per-axis tables, host IEEE double: for every cell (i, j) of the context's stripe, (x_i, y_j) = amb_geometry_position(i, j)
+ * (x depends on i only, y on j only), and
+ *     u_i = (x_i - gt0) / gt1            v_j = (y_j - gt3) / gt5
+ *     covered  iff  0 <= u_i < width  and  0 <= v_j < height          (else: the cell is untouched)
+ *     NEAREST :  c = floor(u_i)                 r = floor(v_j)
+ *     BILINEAR:  s = min(max(u_i - 0.5, 0), width - 1);  c0 = floor(s);  fx = s - c0
+ *                if fx < 2^-20: fx = 0   elif fx > 1 - 2^-20: c0 += 1, fx = 0      (rows alike: t, r0, fy)
+ * Per cell: NEAREST writes p = band[r][c] (its bits) unless p is no-data.  BILINEAR reads only the taps of non-zero
+ * weight: row(r) = fx == 0 ? p(r, c0) : (1-fx) p(r, c0) + fx p(r, c0+1), h = fy == 0 ? row(r0) : (1-fy) row(r0) +
+ * fy row(r0+1), in double, every operation rounded, no FMA contraction; the layer gets (float)h unless a tap it read is
+ * no-data.  So a raster aligned with the map (same resolution, origin on a cell edge) is copied bit for bit by both
+ * methods: importing an exported F32 layer gives the layer back, -0 included.  Cells outside the raster or fed by no-data
+ * keep their value: importing tiles one after another mosaics them.
+ * A NULL pointer, a bad layer or resample, width or height <= 0, a bad row_stride, a geotransform that is not north-up or
+ * not finite, or a device band that is not 4-byte aligned returns AMB_ERR_INVALID_ARGUMENT and writes nothing.  A raster
+ * that does not overlap the stripe returns AMB_OK and copies and writes nothing. */
+typedef enum amb_resample { AMB_RESAMPLE_NEAREST = 0, AMB_RESAMPLE_BILINEAR = 1 } amb_resample;
+/* Host band (pinned or pageable): only the window of rows and columns the stripe reads crosses PCIe; returns when the
+ * band may be reused. */
+int amb_import_raster(amb_ctx* ctx, int layer, const float* host_band, int32_t width, int32_t height, size_t row_stride,
+                      const double gt[6], int has_nodata, float nodata, int resample);
+/* Device band valid on the context's device, read in place; asynchronous on the context's stream. */
+int amb_import_raster_device(amb_ctx* ctx, int layer, const float* device_band, int32_t width, int32_t height,
+                             size_t row_stride, const double gt[6], int has_nodata, float nodata, int resample);
+/* Every stripe of amb_multi imports its own window of the same host band, all devices at once. */
+int amb_multi_import_raster(amb_multi* m, int layer, const float* host_band, int32_t width, int32_t height,
+                            size_t row_stride, const double gt[6], int has_nodata, float nodata, int resample);
+/* Host arithmetic, no GPU: the per-axis tables above for columns [col_begin, col_end) of `geom`.  src_col[rows] / fx[rows]
+ * per cell row i and src_row[n] / fy[n] per column j = col_begin + k (n = col_end - col_begin); an index of -1 marks an
+ * uncovered row or column (NEAREST: the fractions are 0).  What a caller needs to read only the window a stripe uses. */
+int amb_raster_import_tables(const amb_geometry* geom, int32_t col_begin, int32_t col_end, int32_t width, int32_t height,
+                             const double gt[6], int resample, int32_t* src_col, double* fx, int32_t* src_row,
+                             double* fy);
+
 /* ---- measurement ---- */
 int amb_get_timings(amb_ctx* ctx, amb_timings* out);
 
