@@ -152,6 +152,11 @@ SYMBOLS = {
                                           C.c_int, C.c_float, C.c_int]),
     "amb_raster_import_tables": (C.c_int, [C.POINTER(Geometry), C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                            C.POINTER(C.c_double), C.c_int, _P, _P, _P, _P]),
+    "amb_jpeg_max_size": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int, C.c_int, C.c_int, C.c_int32]),
+    "amb_jpeg_encode_device": (C.c_int, [_P, _P, C.c_int32, C.c_int32, C.c_size_t, C.c_int, C.c_int, C.c_int,
+                                         C.c_int32, _P, C.c_size_t, C.POINTER(C.c_size_t)]),
+    "amb_export_jpeg": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int32, _P, C.c_size_t,
+                                  C.POINTER(C.c_size_t)]),
     "amb_get_timings": (C.c_int, [_P, C.POINTER(Timings)]),
     "amb_host_alloc": (C.c_int, [C.POINTER(_P), C.c_size_t]),
     "amb_host_free": (C.c_int, [_P]),

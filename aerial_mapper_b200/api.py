@@ -236,6 +236,27 @@ class GridMap(object):
                                       a.strides[0], gt, 0 if nodata is None else 1,
                                       0.0 if nodata is None else float(nodata), r), ctx)
 
+    def to_jpeg(self, name, quality=95, sampling="420", restart_interval=0, fmt=None):
+        """The context's band of layer `name` as a baseline JPEG file (bytes), exported and encoded on the device
+        (convention: include/aerial_mapper_b200.h, amb_jpeg_sampling), byte for byte cv2.imencode(".jpg", band, params)
+        of the band to_raster(name, fmt) returns.  fmt: "gray8" or "bgr8"; by default "gray8" for `ortho` and "bgr8"
+        for `colored_ortho`, required for any other layer.  sampling: "420" or "444"; restart_interval in MCUs."""
+        if not self._resident:
+            raise AmbError(_lib.AMB_ERR_INVALID_ARGUMENT, "to_jpeg exports device-resident layers: call to_device() first")
+        if fmt is None:
+            fmt = {"ortho": "gray8", "colored_ortho": "bgr8"}.get(name)
+            if fmt is None:
+                raise ValueError("to_jpeg(%r): give fmt='gray8' or fmt='bgr8' for this layer" % (name,))
+        if fmt not in ("gray8", "bgr8"):
+            raise ValueError("to_jpeg: fmt must be 'gray8' or 'bgr8', got %r" % (fmt,))
+        f = _lib.RASTER_FORMAT[fmt]
+        channels = 3 if f == _lib.RASTER_BGR8 else 1
+        args = _jpeg_args(self.geometry.rows, self._col_range[1] - self._col_range[0], channels, quality, sampling,
+                          restart_interval)
+        ctx = self._ctx
+        return _jpeg_call(lambda buf, cap, size: lib().amb_export_jpeg(ctx, LAYER_ID[name], f, *args[3:], buf, cap, size),
+                          args, ctx)
+
     def timings(self):
         t = _lib.Timings()
         check(lib().amb_get_timings(self.context(), C.byref(t)), self._ctx)
@@ -646,3 +667,77 @@ def rectify_stereo_maps(T1_inv, T2_inv, width, height, device=0):
     check(lib().amb_stereo_rectify_maps(int(device), p(T1), p(T2), int(width), int(height), int(width), p(maps[0]),
                                         p(maps[1]), p(maps[2]), p(maps[3])))
     return tuple(maps)
+
+
+# ---- baseline JPEG (amb_jpeg_encode_device, amb_export_jpeg) ----------------------------------------------------------
+JPEG_SAMPLING = {"420": 0, "444": 1}
+
+
+def _jpeg_args(width, height, channels, quality, sampling, restart_interval):
+    """Checks the supported parameter set (ValueError otherwise); returns the C arguments."""
+    if sampling not in JPEG_SAMPLING:
+        raise ValueError("JPEG sampling must be '420' or '444', got %r" % (sampling,))
+    for what, v, lo, hi in (("quality", quality, 1, 100), ("restart_interval", restart_interval, 0, 65535),
+                            ("width", width, 1, 65535), ("height", height, 1, 65535)):
+        if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or not lo <= v <= hi:
+            raise ValueError("JPEG %s must be an integer in [%d, %d], got %r" % (what, lo, hi, v))
+    return (int(width), int(height), channels, int(quality), JPEG_SAMPLING[sampling], int(restart_interval))
+
+
+def _jpeg_call(call, args, ctx):
+    """Runs `call(buffer, capacity, size)`, first with a buffer the size of the raw image, again at the size the library
+    reports if the file is larger (incompressible content); returns the file's bytes."""
+    width, height, channels = args[:3]
+    cap = width * height * channels + 4096
+    for _ in range(2):
+        buf = np.empty(cap, np.uint8)
+        size = C.c_size_t(0)
+        st = call(buf.ctypes.data_as(C.c_void_p), cap, C.byref(size))
+        if st == _lib.AMB_ERR_SIZE_MISMATCH and size.value > cap:
+            cap = size.value
+            continue
+        check(st, ctx)
+        return buf[:size.value].tobytes()
+    raise AmbError(_lib.AMB_ERR_SIZE_MISMATCH, "JPEG size changed between two encodes of the same image")
+
+
+_jpeg_contexts = {}
+
+
+def _jpeg_context(device):
+    """A context per device for encode_jpeg: only its stream and its scratch are used (a 1 x 1 map, no layers)."""
+    ctx = _jpeg_contexts.get(device)
+    if ctx is None:
+        g = Geometry()
+        check(lib().amb_geometry_init(1.0, 1.0, 1.0, 0.0, 0.0, C.byref(g)))
+        ctx = C.c_void_p()
+        check(lib().amb_create(C.byref(g), int(device), 0, 1, C.byref(ctx)))
+        _jpeg_contexts[device] = ctx
+    return ctx
+
+
+def encode_jpeg(image, quality=95, sampling="420", restart_interval=0):
+    """Baseline JPEG (bytes) of a torch CUDA uint8 tensor, H x W (gray) or H x W x 3 (B, G, R), encoded on its device:
+    byte for byte cv2.imencode(".jpg", image, params).  Rows may be padded (a row-sliced view), pixels must be packed.
+    Waits for the work queued on the current torch stream before reading the image."""
+    import torch
+    if not isinstance(image, torch.Tensor) or not image.is_cuda or image.dtype != torch.uint8:
+        raise ValueError("encode_jpeg: expected a torch CUDA uint8 tensor")
+    if image.dim() == 2:
+        channels = 1
+    elif image.dim() == 3 and image.shape[2] == 3:
+        channels = 3
+    else:
+        raise ValueError("encode_jpeg: expected H x W or H x W x 3, got %s" % (tuple(image.shape),))
+    h, w = int(image.shape[0]), int(image.shape[1])
+    inner = (1,) if channels == 1 else (3, 1)
+    if tuple(image.stride())[1:] != inner or (h > 1 and image.stride(0) < w * channels):
+        raise ValueError("encode_jpeg: pixels must be packed along rows, got strides %s" % (tuple(image.stride()),))
+    args = _jpeg_args(w, h, channels, quality, sampling, restart_interval)
+    device = image.device.index if image.device.index is not None else torch.cuda.current_device()
+    ctx = _jpeg_context(device)
+    torch.cuda.current_stream(image.device).synchronize()
+    stride = image.stride(0) if h > 1 else w * channels
+    return _jpeg_call(lambda buf, cap, size: lib().amb_jpeg_encode_device(ctx, C.c_void_p(image.data_ptr()), args[0],
+                                                                          args[1], stride, *args[2:], buf, cap, size),
+                      args, ctx)

@@ -186,6 +186,10 @@ struct amb_ctx {
   amb::DeviceBuffer raster_band;  // amb_export_raster: the converted band before its copy to the host;
                                   // amb_import_raster: the raster window after its copy to the device
   amb::DeviceBuffer raster_taps;  // amb_import_raster*: the per-axis tables of the last import
+  amb::DeviceBuffer jpeg_mcu;     // JPEG encoder (jpeg_encode.cu): DC per block, bit offset per MCU, byte offset per interval
+  amb::DeviceBuffer jpeg_spine;   // ... tile sums of its scans
+  amb::DeviceBuffer jpeg_words;   // ... the entropy-coded stream before byte stuffing, and 0xFF counts per chunk
+  amb::DeviceBuffer jpeg_out;     // ... the stuffed stream with its RST markers, copied to the host
   double dsm_density_hint = 0.0;  // points per cell of the whole cloud (0: derive from the points passed)
   bool dsm_debug = false;
   int dsm_stream_chunks = 4;  // (> 1, only with a host mirror of the output layer) gather + fill in column chunks, each chunk's

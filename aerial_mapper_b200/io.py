@@ -13,6 +13,7 @@ and the output side ("next" row N4):
 and back in: read_geotiff, the DEM GeoTIFFs GDAL writes (GridMap.from_raster resamples them into a layer).
 """
 import math
+import os
 import struct
 import zlib
 
@@ -236,6 +237,26 @@ def write_geotiff(path, raster, geotransform, epsg=32632, nodata=None):
 _TIFF_TYPES = {1: "B", 2: "s", 3: "H", 4: "I", 5: "II", 6: "b", 7: "B", 8: "h", 9: "i", 10: "ii", 11: "f", 12: "d"}
 _SAMPLE_DTYPES = {(8, 1): np.uint8, (16, 2): np.int16, (16, 1): np.uint16, (32, 2): np.int32, (32, 3): np.float32,
                   (64, 3): np.float64}
+
+
+def write_jpeg(path, data, geotransform=None):
+    """Writes the JPEG file `data` (bytes from GridMap.to_jpeg or encode_jpeg) to `path`.  With a GDAL-order
+    geotransform (GridMap.geotransform()) it also writes the ESRI world file next to it (`path` with the extension
+    .jgw): x pixel size, the two rotation terms, y pixel size, then the centre of the top-left pixel (world files
+    locate pixel centres, GDAL geotransforms pixel corners)."""
+    data = bytes(data)
+    if data[:2] != b"\xff\xd8" or data[-2:] != b"\xff\xd9":
+        raise ValueError("write_jpeg: data is not a JPEG file (SOI ... EOI)")
+    if geotransform is not None:
+        gt = [float(v) for v in geotransform]
+        if len(gt) != 6 or not all(math.isfinite(v) for v in gt):
+            raise ValueError("write_jpeg: geotransform must be 6 finite numbers, got %r" % (geotransform,))
+    with open(path, "wb") as f:
+        f.write(data)
+    if geotransform is not None:
+        lines = (gt[1], gt[4], gt[2], gt[5], gt[0] + gt[1] / 2 + gt[2] / 2, gt[3] + gt[4] / 2 + gt[5] / 2)
+        with open(os.path.splitext(path)[0] + ".jgw", "w") as f:
+            f.write("".join("%r\n" % v for v in lines))
 
 
 def _unsupported(tag, value, why):

@@ -492,6 +492,35 @@ int amb_raster_import_tables(const amb_geometry* geom, int32_t col_begin, int32_
                              const double gt[6], int resample, int32_t* src_col, double* fx, int32_t* src_row,
                              double* fy);
 
+/* ---- baseline JPEG of an 8-bit raster ----
+ * Convention.  The file is byte for byte what libjpeg(-turbo) writes (OpenCV cv2.imencode(".jpg", img, params)) for the
+ * same image with its defaults: SOI; APP0 JFIF 1.01, density 1:1 without units; one DQT per table; SOF0 (baseline,
+ * 8 bits); the standard Huffman tables of ITU-T T.81 Annex K as DHT DC0, AC0 (and DC1, AC1 for colour); DRI when the
+ * restart interval is non-zero; one interleaved SOS; the entropy-coded data with RST0..7 markers; EOI.  Arithmetic:
+ * islow integer DCT, quantisation tables of jpeg_set_quality(quality, force_baseline) for luma and chroma alike, and for
+ * colour the 16-bit fixed-point RGB -> YCbCr conversion with, at 4:2:0, 2x2 averaging (bias 1, 2, 1, 2 ... along a row).
+ * Inputs: channels 1 (GRAY8, one component) or 3 (BGR8 as B, G, R bytes, the export's order; YCbCr with three
+ * components), width and height 1..65535, rows `row_stride` >= width * channels bytes apart, any byte alignment;
+ * quality 1..100; sampling AMB_JPEG_420 or AMB_JPEG_444 (ignored for gray); restart_interval 0..65535 MCUs (0: no
+ * restart markers).  Progressive, optimised Huffman tables and other samplings are not offered.
+ * Errors: a NULL pointer, width or height <= 0, or a short row_stride returns AMB_ERR_INVALID_ARGUMENT; a parameter
+ * outside the supported set (a side over 65535, channels, quality, sampling, restart interval) AMB_ERR_UNSUPPORTED.
+ * Neither writes anything. */
+typedef enum amb_jpeg_sampling { AMB_JPEG_420 = 0, AMB_JPEG_444 = 1 } amb_jpeg_sampling;
+/* Host arithmetic, no GPU: an upper bound on the file size (markers and byte stuffing included); 0 if unsupported. */
+size_t amb_jpeg_max_size(int32_t width, int32_t height, int channels, int quality, int sampling,
+                         int32_t restart_interval);
+/* Encodes a device raster valid on the context's device, ordered after earlier work on the context's stream.
+ * Synchronous: on return the *size bytes of the file are in host_out (pinned or pageable).  If capacity < the file's
+ * size it returns AMB_ERR_SIZE_MISMATCH with the size needed in *size and writes nothing to host_out. */
+int amb_jpeg_encode_device(amb_ctx* ctx, const void* d_image, int32_t width, int32_t height, size_t row_stride,
+                           int channels, int quality, int sampling, int32_t restart_interval, void* host_out,
+                           size_t capacity, size_t* size);
+/* amb_export_raster_device of `layer` as AMB_RASTER_GRAY8 or AMB_RASTER_BGR8 into the context's scratch, then
+ * amb_jpeg_encode_device of it: the context's band (image rows [col_begin, col_end)) as an image of its own. */
+int amb_export_jpeg(amb_ctx* ctx, int layer, int format, int quality, int sampling, int32_t restart_interval,
+                    void* host_out, size_t capacity, size_t* size);
+
 /* ---- measurement ---- */
 int amb_get_timings(amb_ctx* ctx, amb_timings* out);
 
