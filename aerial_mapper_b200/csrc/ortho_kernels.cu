@@ -13,6 +13,7 @@
 // compute_view_cone), keeps the survivors as an ascending index list in shared memory, and every thread walks
 // that list reading the per-frame constants (R_C_G, t, camera centre) from __constant__ memory — all threads of
 // a block read the same frame at the same time, i.e. a constant-cache broadcast.
+#include <algorithm>
 #include <cfloat>
 #include <cmath>
 #include <mutex>
@@ -89,15 +90,31 @@ struct OrthoArgs {
   int dominance;                          // 1: per-tile dominance cull of the frame list (needs the inner bounds above)
   const double* exact_data;               // device array [n_frames][8]: inverse(T_G_C) as the reference forms it —
                                           // conjugate quaternion (w, x, y, z), translation -(q^-1).rotate(t), pad
+  // scaling of the guards with the inputs' magnitude (see kDeltaUlps): per tile delta = delta_coef * max(t_max, |X|,
+  // |Y|, |Z| over the tile's cells) bounds |fast - reference| of each camera coordinate
+  double delta_coef;                      // kDeltaUlps * 2^-53 * max(1, |q|^2 over the frames)
+  double t_max;                           // largest |component| of t_G_C and of -R_C_G t_G_C over the frames
+  double px_coef;                         // max(fu, fv) * J: keypoint error <= px_coef * delta / z_c
 };
 
 // Guard bands of the fused fast path.  Its camera coordinates come from a pre-multiplied rotation matrix with FMA
 // contraction and a <= 1 ulp reciprocal; the reference (minkindr / Eigen / aslam_cv2, see exact_* below) rotates by the
-// quaternion formula and divides.  Both carry ~1e-16 relative rounding: keypoints agree to ~1e-12 px (|k| <= 1e4 px),
-// camera z to ~1e-12 m.  A decision closer to its boundary than the guard is re-made with the reference's own
-// operation sequence, un-contracted, so visibility, winner and pixel are the reference's by construction.
-constexpr double kGuardPx = 1e-9;   // keypoint vs raster edge / half-integer
+// quaternion formula and divides.  A decision closer to its boundary than the guard is re-made with the reference's
+// own operation sequence, un-contracted, so visibility, winner and pixel are the reference's by construction.
+// The two sequences round intermediate values as large as the inputs: with M the largest |X|, |Y|, |Z| of the
+// landmark and |t| of the pose, each camera coordinate differs by at most delta = kDeltaUlps * 2^-53 * M.  Counted
+// with unit roundoff u = 2^-53 and |q_i| <= 1: the matrix entries carry <= 16 u each (3 of them per coordinate: 48 u M)
+// and the three FMAs round values <= 2M, 3M, 4M (9 u M), 57 u M for the fast path; the quaternion formula rounds
+// q x v (4 u M, doubled to 8), q x (q x v) (32 u M), the sums (18 u M) and + t (2 u M), 60 u M for the reference.
+// Near the map origin M is ~1e3 m and delta ~1e-11 m; at UTM coordinates (5e6 .. 1e7 m) delta is ~1e-7 m.  The guards:
+//   keypoint: kGuardPx + px_coef * delta / z_c        (u = x/z moves by <= delta (1 + |u|) / z, times the distortion's
+//                                                      row-sum derivative J on the view cone, J including (1 + r_c))
+//   camera z: kGuardZ + delta
+//   sin^2 of the observation angle: the band of the running best + 2 delta / z_c  (|d(z^2/n^2)| <= sqrt(3) delta / n,
+//                                                      n >= z_c), for the candidate and, while pending, for the winner
+constexpr double kGuardPx = 1e-9;   // keypoint vs raster edge / half-integer: rounding of the projection itself
 constexpr double kGuardZ = 1e-6;    // camera z vs kMinimumDepth (1e-10): anything that close to the camera plane goes exact
+constexpr double kDeltaUlps = 128.0;
 
 // ---- the reference's arithmetic, operation by operation (restated third-party code: oracle/thirdparty_math.h cites the
 // upstream sources; parity tests compare with it), no FMA contraction, IEEE division ----
@@ -199,10 +216,13 @@ __device__ __forceinline__ double fast_rcp(double x) {
 
 // aslam::PinholeCamera::project3: rz = 1/z; (u,v) = (x,y)*rz; distort; k = f*u + c.  Returns the reference's
 // keypoint_visible predicate (ortho-backward-grid.cc:164-171): inside the raster and z > 1e-10
-// (POINT_BEHIND_CAMERA is z < 0, PROJECTION_INVALID is 0 <= z <= 1e-10; both rejected).
+// (POINT_BEHIND_CAMERA is z < 0, PROJECTION_INVALID is 0 <= z <= 1e-10; both rejected).  *rzp: the reciprocal of z
+// (of 1e-300 for z <= 0), which scales the guards.
 template <int DIST>
-__device__ __forceinline__ bool project(const OrthoArgs& a, double x, double y, double z, double* kx, double* ky) {
+__device__ __forceinline__ bool project(const OrthoArgs& a, double x, double y, double z, double* kx, double* ky,
+                                        double* rzp) {
   const double rz = fast_rcp(fmax(z, 1e-300));  // 1.0 / z to <= 1 ulp; z <= 1e-10 is rejected below
+  *rzp = rz;
   double u = x * rz;
   double v = y * rz;
   if (DIST == AMB_DIST_RADTAN) {
@@ -369,6 +389,10 @@ __global__ void __launch_bounds__(kOrthoThreads, AMB_OBPS) ortho_kernel_dom(cons
   const double ex = 0.5 * (x_hi - x_lo), ey = 0.5 * (y_hi - y_lo);
   const double ez = 0.5 * (static_cast<double>(zmax) - static_cast<double>(zmin));
   const double rho = sqrt(ex * ex + ey * ey + ez * ez) * (1.0 + 1e-9) + 1e-6;
+  // bound on |fast path - reference| of a camera coordinate over this tile's cells (see kDeltaUlps)
+  const double delta = a.delta_coef * fmax(fmax(a.t_max, fmax(fabs(x_hi), fabs(x_lo))),
+                                           fmax(fmax(fabs(y_hi), fabs(y_lo)),
+                                                static_cast<double>(fmaxf(fabsf(zmin), fabsf(zmax)))));
 
   {
     // The angles are compared through their COSINES (cos is decreasing on [0, pi]), built from the sphere centre's camera
@@ -511,6 +535,10 @@ __global__ void __launch_bounds__(kOrthoThreads, AMB_OBPS) ortho_kernel_dom(cons
   bool check_failed = false;
   unsigned int dirty = 0;  // bit m: a candidate fell inside a band (angle tie / raster edge / camera plane) -> redo exactly
   const double wd = static_cast<double>(a.width), hd = static_cast<double>(a.height);
+  // the guards at this tile's magnitude: per candidate, pixel guard = kGuardPx + gpx_c / z_c, sin^2 band + band_c / z_c
+  const double guard_z = kGuardZ + delta;
+  const double gpx_c = a.px_coef * delta;
+  const double band_c = 2.0 * delta;
 
   // ---- one candidate frame (after the dominance cull: ~4 of 5 tiles at the benchmark geometry) ----
   // The frame loop below projects the winner a second time after its frame loop (like the reference, :186-188) because
@@ -530,14 +558,19 @@ __global__ void __launch_bounds__(kOrthoThreads, AMB_OBPS) ortho_kernel_dom(cons
       double xc = fma(fc.m[1], Y[m], fma(fc.m[2], Z[m], cx));
       double yc = fma(fc.m[4], Y[m], fma(fc.m[5], Z[m], cy));
       double zc = fma(fc.m[7], Y[m], fma(fc.m[8], Z[m], cz));
-      double kx, ky;
-      project<DIST>(a, xc, yc, zc, &kx, &ky);
-      const bool vis = kx >= kGuardPx && ky >= kGuardPx && kx < wd - kGuardPx && ky < hd - kGuardPx && zc > kGuardZ;
-      const bool out = kx < -kGuardPx || ky < -kGuardPx || kx >= wd + kGuardPx || ky >= hd + kGuardPx || zc < -kGuardZ;
+      double kx, ky, rz;
+      project<DIST>(a, xc, yc, zc, &kx, &ky, &rz);
+      const double gpx = fma(gpx_c, rz, kGuardPx);
+      const bool vis = kx >= gpx && ky >= gpx && kx < wd - gpx && ky < hd - gpx && zc > guard_z;
+      const bool out = kx < -gpx || ky < -gpx || kx >= wd + gpx || ky >= hd + gpx || zc < -guard_z;
       const double z2 = zc * zc;
       const double n2 = fma(xc, xc, fma(yc, yc, z2));
-      bool win = vis && (z2 > thr_hi[m] * n2);
-      const bool unc = (vis && !win && (z2 >= thr_lo[m] * n2)) || (!vis && !out);
+      const double en2 = band_c * rz * n2;   // the candidate's own sin^2 error, times n2
+      bool win = vis && (z2 - en2 > thr_hi[m] * n2);
+      const bool unc = (vis && !win && (z2 + en2 >= thr_lo[m] * n2)) || (!vis && !out);
+#ifdef AMB_CUDA_EMU  // tests/emu only: share of cell decisions the guards hand to the exact path
+      emu::note("ortho_exact_decision", unc ? 1 : 0);
+#endif
       bool pend = win;
       float b = best[m];
       if (unc) {  // too close to call: the reference's own operation sequence decides (as in the general path's dirty branch)
@@ -558,7 +591,10 @@ __global__ void __launch_bounds__(kOrthoThreads, AMB_OBPS) ortho_kernel_dom(cons
       const size_t cell = static_cast<size_t>(jl0 + m) * a.rows + i;
       // the pixel is round(keypoint) (:186-193): within the guard of a half-integer (or for a cell that took the exact
       // path) the keypoint is recomputed with the reference's operation sequence
-      const bool near_half = fabs((kx - floor(kx)) - 0.5) < kGuardPx || fabs((ky - floor(ky)) - 0.5) < kGuardPx;
+      const bool near_half = fabs((kx - floor(kx)) - 0.5) < gpx || fabs((ky - floor(ky)) - 0.5) < gpx;
+#ifdef AMB_CUDA_EMU  // tests/emu only: share of winners whose pixel is rounded from the exact keypoint
+      emu::note("ortho_exact_pixel", near_half ? 1 : 0);
+#endif
       if (near_half || unc || !(kx == kx) || !(ky == ky)) {
         exact_to_camera(a, f, X, Y[m], Z[m], &xc, &yc, &zc);
         exact_project<DIST>(a, xc, yc, zc, &kx, &ky);
@@ -598,27 +634,33 @@ __global__ void __launch_bounds__(kOrthoThreads, AMB_OBPS) ortho_kernel_dom(cons
       const double xc = fma(fc.m[1], Y[m], fma(fc.m[2], Z[m], cx));
       const double yc = fma(fc.m[4], Y[m], fma(fc.m[5], Z[m], cy));
       const double zc = fma(fc.m[7], Y[m], fma(fc.m[8], Z[m], cz));
-      double kx, ky;
-      project<DIST>(a, xc, yc, zc, &kx, &ky);
-      // visibility with a guard band (kGuardPx / kGuardZ): certainly inside, certainly not visible, or too close to call
+      double kx, ky, rz;
+      project<DIST>(a, xc, yc, zc, &kx, &ky, &rz);
+      // visibility with a guard band (gpx / guard_z): certainly inside, certainly not visible, or too close to call
       // with FMA-contracted coordinates (NaN keypoints compare false everywhere: too close to call) -> exact path
-      const bool vis = kx >= kGuardPx && ky >= kGuardPx && kx < wd - kGuardPx && ky < hd - kGuardPx && zc > kGuardZ;
-      const bool out = kx < -kGuardPx || ky < -kGuardPx || kx >= wd + kGuardPx || ky >= hd + kGuardPx || zc < -kGuardZ;
+      const double gpx = fma(gpx_c, rz, kGuardPx);
+      const bool vis = kx >= gpx && ky >= gpx && kx < wd - gpx && ky < hd - gpx && zc > guard_z;
+      const bool out = kx < -gpx || ky < -gpx || kx >= wd + gpx || ky >= hd + gpx || zc < -guard_z;
       const double z2 = zc * zc;
       const double n2 = fma(xc, xc, fma(yc, yc, z2));
-      const bool win = vis && (z2 > thr_hi[m] * n2);
+      const double e = band_c * rz;   // bound on this candidate's |sin^2 fast - sin^2 reference|
+      const bool win = vis && (fma(-e, n2, z2) > thr_hi[m] * n2);
       // (cells without an elevation — NaN, or beyond the map edge in a partial tile — have NaN keypoints: never "too
       // close to call", nothing can win there and their layer entries must not even be read)
-      const bool unc = (vis && !win && (z2 >= thr_lo[m] * n2)) || (!vis && !out && ((validmask >> m) & 1u));
+      const bool unc = (vis && !win && (fma(e, n2, z2) >= thr_lo[m] * n2)) || (!vis && !out && ((validmask >> m) & 1u));
       dirty |= (unc ? 1u : 0u) << m;
       const double ref2 = z2 * fast_rcp(n2);
       best_f[m] = win ? f : best_f[m];
-      thr_hi[m] = win ? ref2 + 2e-7 : thr_hi[m];
-      thr_lo[m] = win ? ref2 - 2e-7 : thr_lo[m];
+      thr_hi[m] = win ? ref2 + (2e-7 + e) : thr_hi[m];   // a pending winner's band carries its own error bound too
+      thr_lo[m] = win ? ref2 - (2e-7 + e) : thr_lo[m];
       pending |= (win ? 1u : 0u) << m;
     }
   }
 
+#ifdef AMB_CUDA_EMU
+  for (int m = 0; m < kOStrip; ++m)
+    if ((validmask >> m) & 1u) emu::note("ortho_exact_decision", (dirty >> m) & 1u);
+#endif
   if (dirty) {
     // Rare (a near-tie within the float32 rounding of the running best, a keypoint within 1e-9 px of the raster edge, a
     // landmark on the camera plane): evaluate the reference's recurrence literally for those cells, with the
@@ -652,12 +694,16 @@ __global__ void __launch_bounds__(kOrthoThreads, AMB_OBPS) ortho_kernel_dom(cons
     if (best_f[m] < 0) continue;
     const size_t cell = static_cast<size_t>(jl0 + m) * a.rows + i;
     // the winner's camera coordinates and keypoint, recomputed (the reference projects a second time too, :186-188)
-    double xc, yc, zc, kx, ky;
+    double xc, yc, zc, kx, ky, rz;
     to_camera(best_f[m], X, Y[m], Z[m], &xc, &yc, &zc);
-    project<DIST>(a, xc, yc, zc, &kx, &ky);
+    project<DIST>(a, xc, yc, zc, &kx, &ky, &rz);
     // the pixel is round(keypoint) (:186-193): within the guard of a half-integer (or for a cell that already took the
     // exact path) the keypoint is recomputed with the reference's operation sequence
-    const bool near_half = fabs((kx - floor(kx)) - 0.5) < kGuardPx || fabs((ky - floor(ky)) - 0.5) < kGuardPx;
+    const double gpx = fma(gpx_c, rz, kGuardPx);
+    const bool near_half = fabs((kx - floor(kx)) - 0.5) < gpx || fabs((ky - floor(ky)) - 0.5) < gpx;
+#ifdef AMB_CUDA_EMU
+    emu::note("ortho_exact_pixel", near_half ? 1 : 0);
+#endif
     if (near_half || ((dirty >> m) & 1u) || !(kx == kx) || !(ky == ky)) {
       exact_to_camera(a, best_f[m], X, Y[m], Z[m], &xc, &yc, &zc);
       exact_project<DIST>(a, xc, yc, zc, &kx, &ky);
@@ -869,6 +915,32 @@ bool compute_view_rect(const amb_camera& cam, double rc, double* u_lo, double* u
   return cam.fu > 0.0 && cam.fv > 0.0;
 }
 
+// Bound J on how far a keypoint moves, in units of f, per unit of camera-coordinate error times z_c, for rays with
+// undistorted normalised radius <= r: |du|, |dv| <= delta (1 + r) / z_c, and a row of the distortion's Jacobian sums to
+// at most the bound below (rad-tan: differentiate u (1 + k1 rho^2 + k2 rho^4) + 2 p1 u v + p2 (rho^2 + 2 u^2); equidistant:
+// D = u theta_d(theta) / r with theta = atan(r), |theta_d / r| <= P and |d theta_d / d theta| <= Q; FOV: D = u s(r)
+// with |s| <= 2 tan(w/2) / w and |r s'| <= 2 |s|).
+double distortion_slope(const amb_camera& cam, double r) {
+  const double* k = cam.dist;
+  double J = 1.0;
+  if (cam.dist_type == AMB_DIST_RADTAN) {
+    J = 1.0 + 5.0 * std::fabs(k[0]) * r * r + 9.0 * std::fabs(k[1]) * r * r * r * r +
+        8.0 * (std::fabs(k[2]) + std::fabs(k[3])) * r;
+  } else if (cam.dist_type == AMB_DIST_EQUIDISTANT) {
+    const double t2 = std::atan(r) * std::atan(r);
+    const double P = 1.0 + std::fabs(k[0]) * t2 + std::fabs(k[1]) * t2 * t2 + std::fabs(k[2]) * t2 * t2 * t2 +
+                     std::fabs(k[3]) * t2 * t2 * t2 * t2;
+    const double Q = 1.0 + 3.0 * std::fabs(k[0]) * t2 + 5.0 * std::fabs(k[1]) * t2 * t2 +
+                     7.0 * std::fabs(k[2]) * t2 * t2 * t2 + 9.0 * std::fabs(k[3]) * t2 * t2 * t2 * t2;
+    J = 3.0 * P + 2.0 * Q;
+  } else if (cam.dist_type == AMB_DIST_FOV) {
+    const double w = k[0];
+    const double s = (w * w < 1e-5) ? 1.0 : std::fabs(2.0 * std::tan(w / 2.) / w);
+    J = 4.0 * std::max(1.0, s);
+  }
+  return J * (1.0 + r);
+}
+
 }  // namespace
 
 // d_images != nullptr: frames resident in HBM -> one fused kernel per chunk of frames.
@@ -916,6 +988,7 @@ int ortho_run(amb_ctx* ctx, const amb_camera* camera, const double* T_G_B, const
   FrameConst* fcs = stage.take<FrameConst>(n);
   double* cull = stage.take<double>(12 * n);
   double* exact = stage.take<double>(8 * n);
+  double q_norm2 = 1.0, t_max = 0.0;   // magnitudes the guards scale with (kDeltaUlps)
   for (size_t f = 0; f < n; ++f) {
     const double* p = T_G_B + 7 * f;
     const Quat q_G_B = {p[3], p[4], p[5], p[6]};
@@ -939,6 +1012,9 @@ int ortho_run(amb_ctx* ctx, const amb_camera* camera, const double* T_G_B, const
     double* ef = &exact[8 * f];
     ef[0] = qi.w; ef[1] = qi.x; ef[2] = qi.y; ef[3] = qi.z;
     ef[4] = -ti.x; ef[5] = -ti.y; ef[6] = -ti.z; ef[7] = 0.0;
+    q_norm2 = std::max(q_norm2, q.w * q.w + q.x * q.x + q.y * q.y + q.z * q.z);
+    t_max = std::max({t_max, std::fabs(t.x), std::fabs(t.y), std::fabs(t.z), std::fabs(ti.x), std::fabs(ti.y),
+                      std::fabs(ti.z)});
   }
 
   AMB_CUDA(ctx, ctx->frame_table.reserve(n * sizeof(uint8_t*)));
@@ -1009,6 +1085,11 @@ int ortho_run(amb_ctx* ctx, const amb_camera* camera, const double* T_G_B, const
     a.nv_lo = std::sqrt(1.0 + a.v_lo * a.v_lo);
     a.nv_hi = std::sqrt(1.0 + a.v_hi * a.v_hi);
   }
+  // guards scaled with the inputs' magnitude; without a view cone the normalised radius of an imaged ray is bounded by
+  // nothing better than the cone scan's limit
+  a.delta_coef = kDeltaUlps * std::ldexp(1.0, -53) * q_norm2;
+  a.t_max = t_max;
+  a.px_coef = std::max(std::fabs(camera->fu), std::fabs(camera->fv)) * distortion_slope(*camera, a.cone ? tc : 1.0e3);
 
   // Dominance cull (amb_ortho_set_dominance_cull): needs an INNER bound, a set of rays that are certainly imaged inside
   // the raster.  r_in: normalised distance from the principal point to the nearest raster edge.

@@ -1,5 +1,6 @@
 """Randomised cases of the orthomosaic kernels, plain and with the dominance cull on the CPU EMULATION of the kernel source (tests/emu) against the oracle:
-sizes from 1x1, every distortion model / radius / density / offset the generators below draw.  No GPU involved.
+sizes from 1x1, every distortion model / radius / density / offset the generators below draw, the map at the origin or at
+UTM coordinates (northern and southern hemisphere).  No GPU involved.
 
     python tools/emu_fuzz_ortho.py <seed> <cases>      # exits non-zero on any mismatch
 """
@@ -15,6 +16,9 @@ from oracle import pyoracle as po
 from common import ulp_diff, fresh_layers
 from scipy.spatial.transform import Rotation as R
 rng = np.random.default_rng(int(sys.argv[1]) if len(sys.argv) > 1 else 0)
+# map positions from their own stream, so that a seed draws the same scenes as before positions were drawn
+pos_rng = np.random.default_rng([int(sys.argv[1]) if len(sys.argv) > 1 else 0, 1])
+POSITIONS = ((0.0, 0.0), (4.6e5 + 123.0, 5.2e6 + 457.0), (4.6e5 + 321.0, 9.9e6 + 211.0))
 fails = 0
 checked = 0
 t0 = time.time()
@@ -35,6 +39,9 @@ for it in range(N):
     lines, per = int(rng.integers(1, 5)), int(rng.integers(1, 7))
     poses = synth.lawnmower_poses(lines, per, rows * res / 2, cols * res / 2, agl, int(rng.integers(0, 1000)), jitter_pos=agl / 50,
                                   jitter_rp_deg=float(rng.choice([1.0, 5.0, 20.0])))
+    pos = POSITIONS[int(pos_rng.integers(0, len(POSITIONS)))]
+    poses[:, 0] += pos[0]
+    poses[:, 1] += pos[1]
     ch = 3 if colored else 1
     imgs = [synth.procedural_image(k, camd["width"], camd["height"], ch) for k in range(len(poses))]
     elev = synth.analytic_elevation(rows, cols, res)
@@ -45,7 +52,7 @@ for it in range(N):
     outs = []
     for dom in ("0", "1"):
         os.environ["AMB_ORTHO_DOMINANCE"] = dom
-        gm = amb.AerialGridMap(amb.GridMapSettings(0, 0, rows * res, cols * res, res)).getMutable()
+        gm = amb.AerialGridMap(amb.GridMapSettings(pos[0], pos[1], rows * res, cols * res, res)).getMutable()
         if gm.getSize() != (rows, cols): break
         gm["elevation"] = elev
         if prior:
@@ -61,13 +68,13 @@ for it in range(N):
     checked += 1
     L = fresh_layers(rows, cols, elev)
     if prior: L["elevation_angle"][...] = np.float32(1.2)
-    st, _ = po.ortho_process(po.make_geometry(rows, cols, res), L, po.make_camera(**camd), poses, imgs, colored=colored, num_threads=-1)
+    st, _ = po.ortho_process(po.make_geometry(rows, cols, res, pos[0], pos[1]), L, po.make_camera(**camd), poses, imgs, colored=colored, num_threads=-1)
     key = "colored_ortho" if colored else "ortho"
     for nm, g in zip(("plain", "dom"), outs):
         ok = st == 0 and np.array_equal(g["observation_index"], L["observation_index"], equal_nan=True) and \
             np.array_equal(g[key].view(np.uint32), L[key].view(np.uint32)) and ulp_diff(g["elevation_angle"], L["elevation_angle"]).max() <= 1
         if not ok:
             fails += 1
-            print("MISMATCH", nm, "it", it, (rows, cols, res, dist_type, dist, colored, scale, agl, lines, per, prior), "st", st)
+            print("MISMATCH", nm, "it", it, (rows, cols, res, pos, dist_type, dist, colored, scale, agl, lines, per, prior), "st", st)
 print("done", N, "cases,", checked, "checked, fails", fails, "%.0fs" % (time.time() - t0))
 sys.exit(1 if fails or checked < N // 2 else 0)
