@@ -330,6 +330,13 @@ class Dsm(object):
         # chunked evaluation + early mirroring of finished columns (amb_dsm_set_stream_chunks); 1 = off, default 4
         self.stream_chunks = max(1, int(os.environ.get("AMB_DSM_STREAM_CHUNKS", "4") or 4))
 
+    def _configure(self, ctx):
+        """This Dsm's debug, stream_chunks and precision onto the map's context, before each of its calls."""
+        check(lib().amb_dsm_enable_debug(ctx, 1 if self.debug else 0), ctx)
+        check(lib().amb_dsm_set_stream_chunks(ctx, int(self.stream_chunks)), ctx)
+        if self.precision is not None:
+            check(lib().amb_dsm_set_precision(ctx, _lib.DSM_F32 if self.precision == "f32" else _lib.DSM_F64), ctx)
+
     def process(self, point_cloud, map):
         """point_cloud: float64 [n, 3] (the AoS layout of std::vector<Eigen::Vector3d>).  Mutates map['elevation']."""
         pc = np.ascontiguousarray(point_cloud, dtype=np.float64)
@@ -343,10 +350,7 @@ class Dsm(object):
         s = self.settings_
         if not map.is_resident():
             map.upload(("elevation",))
-        check(lib().amb_dsm_enable_debug(ctx, 1 if self.debug else 0), ctx)
-        check(lib().amb_dsm_set_stream_chunks(ctx, int(self.stream_chunks)), ctx)
-        if self.precision is not None:
-            check(lib().amb_dsm_set_precision(ctx, _lib.DSM_F32 if self.precision == "f32" else _lib.DSM_F64), ctx)
+        self._configure(ctx)
         check(lib().amb_dsm_process(ctx, pc.ctypes.data_as(C.c_void_p), n, int(s.interpolation_radius),
                                     float(s.center_easting), float(s.center_northing)), ctx)
         self._fetch_debug(map)
@@ -361,10 +365,7 @@ class Dsm(object):
             return
         ctx = map.context()
         s = self.settings_
-        check(lib().amb_dsm_enable_debug(ctx, 1 if self.debug else 0), ctx)
-        check(lib().amb_dsm_set_stream_chunks(ctx, int(self.stream_chunks)), ctx)
-        if self.precision is not None:
-            check(lib().amb_dsm_set_precision(ctx, _lib.DSM_F32 if self.precision == "f32" else _lib.DSM_F64), ctx)
+        self._configure(ctx)
         if d_ids is None:
             check(lib().amb_dsm_process_device(ctx, C.c_void_p(int(d_xyz)), int(n), int(s.interpolation_radius),
                                                float(s.center_easting), float(s.center_northing)), ctx)
@@ -380,9 +381,7 @@ class Dsm(object):
         asynchronous — map.sync() before reading results."""
         ctx = map.context()
         s = self.settings_
-        check(lib().amb_dsm_enable_debug(ctx, 1 if self.debug else 0), ctx)
-        if self.precision is not None:
-            check(lib().amb_dsm_set_precision(ctx, _lib.DSM_F32 if self.precision == "f32" else _lib.DSM_F64), ctx)
+        self._configure(ctx)
         check(lib().amb_dsm_process_sharded_device(ctx, C.c_void_p(int(d_xyz)), C.c_void_p(int(d_ids)), int(n_local),
                                                    int(s.interpolation_radius), float(s.center_easting),
                                                    float(s.center_northing), int(halo_capacity)), ctx)
@@ -394,8 +393,7 @@ class Dsm(object):
         n = pc.size // 3
         ctx = map.context()
         s = self.settings_
-        if self.precision is not None:
-            check(lib().amb_dsm_set_precision(ctx, _lib.DSM_F32 if self.precision == "f32" else _lib.DSM_F64), ctx)
+        self._configure(ctx)
         check(lib().amb_dsm_process_sharded(ctx, pc.ctypes.data_as(C.c_void_p), idv.ctypes.data_as(C.c_void_p), n,
                                             int(s.interpolation_radius), float(s.center_easting),
                                             float(s.center_northing), int(halo_capacity)), ctx)

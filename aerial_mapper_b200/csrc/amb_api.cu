@@ -109,6 +109,94 @@ static int finish_flags(amb_ctx* ctx, unsigned int offset_words, int err_code) {
   return err_code;
 }
 
+// One Dsm::process / OrthoFromPcl::process, wherever its inputs live: every amb_dsm_process* and
+// amb_ortho_from_pcl_process* entry point is one call of run_cloud.
+struct CloudCall {
+  int mode = 0;           // 0 Dsm (elevation), 1 OrthoFromPcl (ortho): dsm_run's mode
+  bool host = false;      // inputs in host memory: uploaded here, the call is synchronous
+  bool sharded = false;   // a rank's share of a sharded cloud (the *_sharded* entry points)
+  bool need_ids = false;  // NULL ids are rejected (sharded clouds, amb_ortho_from_pcl_process_device_ids)
+  const double* xyz = nullptr;
+  const int32_t* intensities = nullptr;  // mode 1 only
+  const uint64_t* ids = nullptr;         // NULL: array positions are the canonical order
+  size_t n = 0;
+  int32_t radius = 0;
+  double center_easting = 0.0, center_northing = 0.0;  // mode 0 only
+  int32_t adaptive = 0;        // mode 1, not sharded: ortho-from-pcl.cc:63-72 (pcl_adaptive_kernels.cu)
+  uint32_t halo_capacity = 0;  // sharded only
+};
+
+static int run_cloud(amb_ctx* ctx, const CloudCall& c) {
+  if (!ctx) return AMB_ERR_INVALID_ARGUMENT;
+  if (c.need_ids && !c.ids) return AMB_ERR_INVALID_ARGUMENT;
+  const bool inputs = c.xyz && (c.mode == 0 || c.intensities);
+  // A rank of a communicator may own no points of a sharded cloud, so its other arguments are checked before n and its
+  // empty share still takes part in the exchange.  Without a communicator the share is the whole cloud.
+  const bool exchange = c.sharded && ctx->comm_size > 1 && ctx->nccl_comm;
+  if (c.sharded && (!inputs || c.radius < 1)) return AMB_ERR_INVALID_ARGUMENT;
+  if (c.n == 0 && !exchange) return AMB_ERR_EMPTY;  // dsm.cc:189-192, CHECK(!pointcloud.empty()) ortho-from-pcl.cc:23
+  if (!inputs) return AMB_ERR_INVALID_ARGUMENT;
+  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
+
+  const double* xyz = c.xyz;
+  const int* intensities = c.mode == 1 ? c.intensities : nullptr;
+  const unsigned long long* ids = reinterpret_cast<const unsigned long long*>(c.ids);
+  // The upload of a whole cloud is the "h2d" phase of the call's timings.  A sharded share is uploaded before the
+  // timed region, whose "h2d" phase is the halo exchange (sharded_step); its buffers are never empty, so that a rank
+  // without points still passes valid device pointers to the exchange.
+  const bool timed_upload = c.host && !c.sharded;
+  if (c.host) {
+    const size_t cap = c.sharded ? std::max<size_t>(c.n, 1) : c.n;
+    AMB_CUDA(ctx, ctx->points.reserve(cap * 3 * sizeof(double)));
+    if (c.mode == 1) AMB_CUDA(ctx, ctx->intensities.reserve(cap * sizeof(int32_t)));
+    if (c.sharded) AMB_CUDA(ctx, ctx->point_ids.reserve(cap * sizeof(uint64_t)));
+    if (timed_upload) AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_BEGIN], ctx->stream));
+    if (c.n) {
+      const int st = staged_h2d(ctx, ctx->points.ptr, c.xyz, c.n * 3 * sizeof(double), ctx->stream);  // pageable clouds
+      if (st != AMB_OK) return st;
+      if (c.mode == 1)
+        AMB_CUDA(ctx, cudaMemcpyAsync(ctx->intensities.ptr, c.intensities, c.n * sizeof(int32_t), cudaMemcpyHostToDevice,
+                                      ctx->stream));
+      if (c.sharded)
+        AMB_CUDA(ctx, cudaMemcpyAsync(ctx->point_ids.ptr, c.ids, c.n * sizeof(uint64_t), cudaMemcpyHostToDevice,
+                                      ctx->stream));
+    }
+    xyz = ctx->points.as<double>();
+    if (c.mode == 1) intensities = ctx->intensities.as<int>();
+    if (c.sharded) ids = ctx->point_ids.as<unsigned long long>();
+    if (timed_upload) AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_H2D_END], ctx->stream));
+  }
+
+  int st;
+  if (exchange) {
+    // records its own events and sets dsm_timed
+    st = sharded_step(ctx, xyz, intensities, reinterpret_cast<const uint64_t*>(ids), c.n, c.radius, c.center_easting,
+                      c.center_northing, c.halo_capacity, c.mode);
+  } else {
+    if (!timed_upload) {  // inputs already on the device: an empty "h2d" phase
+      AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_BEGIN], ctx->stream));
+      AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_H2D_END], ctx->stream));
+    }
+    ctx->dsm_had_h2d = timed_upload;
+    float* saved = nullptr;
+    if (c.adaptive) {
+      const int pst = pcl_adaptive_prepare(ctx, &saved);
+      if (pst != AMB_OK)  // frees what prepare made; no pass ran, so the timings of the previous call stay
+        return pcl_adaptive_finish(ctx, pst, xyz, ids, intensities, c.n, c.radius, saved);
+    }
+    st = dsm_run(ctx, xyz, ids, c.n, c.radius, c.center_easting, c.center_northing, c.mode, intensities);
+    if (c.adaptive) st = pcl_adaptive_finish(ctx, st, xyz, ids, intensities, c.n, c.radius, saved);
+    ctx->dsm_timed = (st == AMB_OK);
+  }
+  if (st != AMB_OK || !c.host) return st;
+  // Host entry points return with their result final on the device.  amb_dsm_process also reports a point on a cell
+  // centre at once, as the reference's Dsm::process does (CHECK in dsm.cc); the other host entry points leave their
+  // sticky flags to amb_sync.
+  if (c.mode == 0 && !c.sharded) return finish_flags(ctx, CTR_DSM_COINCIDENT, AMB_ERR_COINCIDENT_POINT);
+  AMB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return AMB_OK;
+}
+
 }  // namespace amb
 
 using namespace amb;
@@ -343,72 +431,72 @@ int amb_layer_device_ptr(amb_ctx* ctx, int layer, float** device_slab) {
   return AMB_OK;
 }
 
-// ---- DSM ----
+// ---- DSM and OrthoFromPcl ("next" row N1, SURVEY.md §8f) ----
+int amb_dsm_process(amb_ctx* ctx, const double* xyz, size_t n, int32_t interpolation_radius,
+                    double center_easting, double center_northing) {
+  return run_cloud(ctx, {.mode = 0, .host = true, .xyz = xyz, .n = n, .radius = interpolation_radius,
+                         .center_easting = center_easting, .center_northing = center_northing});
+}
+
 int amb_dsm_process_device(amb_ctx* ctx, const double* d_xyz, size_t n, int32_t interpolation_radius,
                            double center_easting, double center_northing) {
-  if (!ctx) return AMB_ERR_INVALID_ARGUMENT;
-  if (n == 0) return AMB_ERR_EMPTY;  // dsm.cc:189-192
-  if (!d_xyz) return AMB_ERR_INVALID_ARGUMENT;
-  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
-  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_BEGIN], ctx->stream));
-  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_H2D_END], ctx->stream));
-  ctx->dsm_had_h2d = false;
-  int st = dsm_run(ctx, d_xyz, nullptr, n, interpolation_radius, center_easting, center_northing);
-  ctx->dsm_timed = (st == AMB_OK);
-  return st;
+  return run_cloud(ctx, {.mode = 0, .xyz = d_xyz, .n = n, .radius = interpolation_radius,
+                         .center_easting = center_easting, .center_northing = center_northing});
 }
 
 int amb_dsm_process_device_ids(amb_ctx* ctx, const double* d_xyz, const uint64_t* d_ids, size_t n,
                                int32_t interpolation_radius, double center_easting, double center_northing) {
-  if (!ctx) return AMB_ERR_INVALID_ARGUMENT;
-  if (n == 0) return AMB_ERR_EMPTY;
-  if (!d_xyz) return AMB_ERR_INVALID_ARGUMENT;
-  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
-  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_BEGIN], ctx->stream));
-  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_H2D_END], ctx->stream));
-  ctx->dsm_had_h2d = false;
-  int st = dsm_run(ctx, d_xyz, reinterpret_cast<const unsigned long long*>(d_ids), n, interpolation_radius,
-                   center_easting, center_northing);
-  ctx->dsm_timed = (st == AMB_OK);
-  return st;
+  return run_cloud(ctx, {.mode = 0, .xyz = d_xyz, .ids = d_ids, .n = n, .radius = interpolation_radius,
+                         .center_easting = center_easting, .center_northing = center_northing});
 }
 
-// ---- OrthoFromPcl ("next" row N1, SURVEY.md §8f) ----
-// d_ids: nullptr (array positions are the canonical order) or the caller's global point ids
-static int ortho_from_pcl_device(amb_ctx* ctx, const double* d_xyz, const int32_t* d_intensities,
-                                 const unsigned long long* d_ids, size_t n, int32_t interpolation_radius,
-                                 int32_t use_adaptive_interpolation) {
-  if (!ctx) return AMB_ERR_INVALID_ARGUMENT;
-  if (n == 0) return AMB_ERR_EMPTY;  // CHECK(!pointcloud.empty()), ortho-from-pcl.cc:23
-  if (!d_xyz || !d_intensities) return AMB_ERR_INVALID_ARGUMENT;
-  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
-  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_BEGIN], ctx->stream));
-  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_H2D_END], ctx->stream));
-  ctx->dsm_had_h2d = false;
-  float* saved = nullptr;  // adaptive interpolation (ortho-from-pcl.cc:63-72): pcl_adaptive_kernels.cu
-  if (use_adaptive_interpolation) {
-    const int pst = pcl_adaptive_prepare(ctx, &saved);
-    if (pst != AMB_OK)
-      return pcl_adaptive_finish(ctx, pst, d_xyz, d_ids, d_intensities, n, interpolation_radius, saved);
-  }
-  int st = dsm_run(ctx, d_xyz, d_ids, n, interpolation_radius, 0.0, 0.0, 1, d_intensities);
-  if (use_adaptive_interpolation)
-    st = pcl_adaptive_finish(ctx, st, d_xyz, d_ids, d_intensities, n, interpolation_radius, saved);
-  ctx->dsm_timed = (st == AMB_OK);
-  return st;
+int amb_dsm_process_sharded(amb_ctx* ctx, const double* xyz, const uint64_t* ids, size_t n_local,
+                            int32_t interpolation_radius, double center_easting, double center_northing,
+                            uint32_t halo_capacity) {
+  return run_cloud(ctx, {.mode = 0, .host = true, .sharded = true, .need_ids = true, .xyz = xyz, .ids = ids,
+                         .n = n_local, .radius = interpolation_radius, .center_easting = center_easting,
+                         .center_northing = center_northing, .halo_capacity = halo_capacity});
+}
+
+int amb_dsm_process_sharded_device(amb_ctx* ctx, const double* d_xyz, const uint64_t* d_ids, size_t n_local,
+                                   int32_t interpolation_radius, double center_easting, double center_northing,
+                                   uint32_t halo_capacity) {
+  return run_cloud(ctx, {.mode = 0, .sharded = true, .need_ids = true, .xyz = d_xyz, .ids = d_ids, .n = n_local,
+                         .radius = interpolation_radius, .center_easting = center_easting,
+                         .center_northing = center_northing, .halo_capacity = halo_capacity});
+}
+
+int amb_ortho_from_pcl_process(amb_ctx* ctx, const double* xyz, const int32_t* intensities, size_t n,
+                               int32_t interpolation_radius, int32_t use_adaptive_interpolation) {
+  return run_cloud(ctx, {.mode = 1, .host = true, .xyz = xyz, .intensities = intensities, .n = n,
+                         .radius = interpolation_radius, .adaptive = use_adaptive_interpolation});
 }
 
 int amb_ortho_from_pcl_process_device(amb_ctx* ctx, const double* d_xyz, const int32_t* d_intensities, size_t n,
                                       int32_t interpolation_radius, int32_t use_adaptive_interpolation) {
-  return ortho_from_pcl_device(ctx, d_xyz, d_intensities, nullptr, n, interpolation_radius, use_adaptive_interpolation);
+  return run_cloud(ctx, {.mode = 1, .xyz = d_xyz, .intensities = d_intensities, .n = n,
+                         .radius = interpolation_radius, .adaptive = use_adaptive_interpolation});
 }
 
 int amb_ortho_from_pcl_process_device_ids(amb_ctx* ctx, const double* d_xyz, const int32_t* d_intensities,
                                           const uint64_t* d_ids, size_t n, int32_t interpolation_radius,
                                           int32_t use_adaptive_interpolation) {
-  if (!d_ids) return AMB_ERR_INVALID_ARGUMENT;
-  return ortho_from_pcl_device(ctx, d_xyz, d_intensities, reinterpret_cast<const unsigned long long*>(d_ids), n,
-                               interpolation_radius, use_adaptive_interpolation);
+  return run_cloud(ctx, {.mode = 1, .need_ids = true, .xyz = d_xyz, .intensities = d_intensities, .ids = d_ids,
+                         .n = n, .radius = interpolation_radius, .adaptive = use_adaptive_interpolation});
+}
+
+int amb_ortho_from_pcl_process_sharded(amb_ctx* ctx, const double* xyz, const int32_t* intensities, const uint64_t* ids,
+                                       size_t n_local, int32_t interpolation_radius, uint32_t halo_capacity) {
+  return run_cloud(ctx, {.mode = 1, .host = true, .sharded = true, .need_ids = true, .xyz = xyz,
+                         .intensities = intensities, .ids = ids, .n = n_local, .radius = interpolation_radius,
+                         .halo_capacity = halo_capacity});
+}
+
+int amb_ortho_from_pcl_process_sharded_device(amb_ctx* ctx, const double* d_xyz, const int32_t* d_intensities,
+                                              const uint64_t* d_ids, size_t n_local, int32_t interpolation_radius,
+                                              uint32_t halo_capacity) {
+  return run_cloud(ctx, {.mode = 1, .sharded = true, .need_ids = true, .xyz = d_xyz, .intensities = d_intensities,
+                         .ids = d_ids, .n = n_local, .radius = interpolation_radius, .halo_capacity = halo_capacity});
 }
 
 int amb_ortho_from_pcl_extract_halo(amb_ctx* ctx, const double* d_xyz, const int32_t* d_intensities,
@@ -421,41 +509,6 @@ int amb_ortho_from_pcl_extract_halo(amb_ctx* ctx, const double* d_xyz, const int
   return dsm_extract_halo(ctx, d_xyz, reinterpret_cast<const unsigned long long*>(d_ids), n, y_lo, y_hi, reach, 0.0,
                           d_out_xyz, reinterpret_cast<unsigned long long*>(d_out_ids), capacity, d_count, d_intensities,
                           d_out_intensities);
-}
-
-int amb_ortho_from_pcl_process(amb_ctx* ctx, const double* xyz, const int32_t* intensities, size_t n,
-                               int32_t interpolation_radius, int32_t use_adaptive_interpolation) {
-  if (!ctx) return AMB_ERR_INVALID_ARGUMENT;
-  if (n == 0) return AMB_ERR_EMPTY;
-  if (!xyz || !intensities) return AMB_ERR_INVALID_ARGUMENT;
-  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
-  AMB_CUDA(ctx, ctx->points.reserve(n * 3 * sizeof(double)));
-  AMB_CUDA(ctx, ctx->intensities.reserve(n * sizeof(int32_t)));
-  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_BEGIN], ctx->stream));
-  {
-    const int sst = staged_h2d(ctx, ctx->points.ptr, xyz, n * 3 * sizeof(double), ctx->stream);
-    if (sst != AMB_OK) return sst;
-  }
-  AMB_CUDA(ctx, cudaMemcpyAsync(ctx->intensities.ptr, intensities, n * sizeof(int32_t), cudaMemcpyHostToDevice,
-                                ctx->stream));
-  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_H2D_END], ctx->stream));
-  ctx->dsm_had_h2d = true;
-  float* saved = nullptr;
-  if (use_adaptive_interpolation) {
-    const int pst = pcl_adaptive_prepare(ctx, &saved);
-    if (pst != AMB_OK)
-      return pcl_adaptive_finish(ctx, pst, ctx->points.as<double>(), nullptr, ctx->intensities.as<int>(), n,
-                                 interpolation_radius, saved);
-  }
-  int st = dsm_run(ctx, ctx->points.as<double>(), nullptr, n, interpolation_radius, 0.0, 0.0, 1,
-                   ctx->intensities.as<int>());
-  if (use_adaptive_interpolation)
-    st = pcl_adaptive_finish(ctx, st, ctx->points.as<double>(), nullptr, ctx->intensities.as<int>(), n,
-                             interpolation_radius, saved);
-  ctx->dsm_timed = (st == AMB_OK);
-  if (st != AMB_OK) return st;
-  AMB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return AMB_OK;
 }
 
 int amb_dsm_set_stream_chunks(amb_ctx* ctx, int chunks) {
@@ -506,24 +559,6 @@ int amb_dsm_extract_halo(amb_ctx* ctx, const double* d_xyz, const uint64_t* d_id
   return dsm_extract_halo(ctx, d_xyz, reinterpret_cast<const unsigned long long*>(d_ids), n, y_lo, y_hi, reach,
                           center_easting, d_out_xyz, reinterpret_cast<unsigned long long*>(d_out_ids), capacity,
                           d_count);
-}
-
-int amb_dsm_process(amb_ctx* ctx, const double* xyz, size_t n, int32_t interpolation_radius,
-                    double center_easting, double center_northing) {
-  if (!ctx) return AMB_ERR_INVALID_ARGUMENT;
-  if (n == 0) return AMB_ERR_EMPTY;
-  if (!xyz) return AMB_ERR_INVALID_ARGUMENT;
-  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
-  AMB_CUDA(ctx, ctx->points.reserve(n * 3 * sizeof(double)));
-  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_BEGIN], ctx->stream));
-  int st = staged_h2d(ctx, ctx->points.ptr, xyz, n * 3 * sizeof(double), ctx->stream);  // (pageable clouds: host_staging.cu)
-  if (st != AMB_OK) return st;
-  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_H2D_END], ctx->stream));
-  ctx->dsm_had_h2d = true;
-  st = dsm_run(ctx, ctx->points.as<double>(), nullptr, n, interpolation_radius, center_easting, center_northing);
-  ctx->dsm_timed = (st == AMB_OK);
-  if (st != AMB_OK) return st;
-  return finish_flags(ctx, CTR_DSM_COINCIDENT, AMB_ERR_COINCIDENT_POINT);
 }
 
 int amb_dsm_enable_debug(amb_ctx* ctx, int enable) {

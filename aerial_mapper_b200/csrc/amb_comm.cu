@@ -403,9 +403,9 @@ namespace amb {
 // The sharded step shared by Dsm (mode 0) and OrthoFromPcl (mode 1, d_intensities: every record's z is the point's
 // intensity, no centre shift): exchange of the border halos, then the binning over [own points | neighbours' halos].
 // The caller has checked the arguments and that the context belongs to a communicator of several ranks.
-static int sharded_step(amb_ctx* ctx, const double* d_xyz, const int* d_intensities, const uint64_t* d_ids,
-                        size_t n_local, int32_t interpolation_radius, double center_easting, double center_northing,
-                        uint32_t halo_capacity, int mode) {
+int sharded_step(amb_ctx* ctx, const double* d_xyz, const int* d_intensities, const uint64_t* d_ids,
+                 size_t n_local, int32_t interpolation_radius, double center_easting, double center_northing,
+                 uint32_t halo_capacity, int mode) {
   if (halo_capacity == 0) return AMB_ERR_INVALID_ARGUMENT;
   const int nranks = ctx->comm_size, rank = ctx->comm_rank;
   const size_t seg_bytes = 32 * (static_cast<size_t>(halo_capacity) + 1);  // header + records
@@ -538,76 +538,3 @@ static int sharded_step(amb_ctx* ctx, const double* d_xyz, const int* d_intensit
 }
 
 }  // namespace amb
-
-extern "C" {
-
-int amb_dsm_process_sharded_device(amb_ctx* ctx, const double* d_xyz, const uint64_t* d_ids, size_t n_local,
-                                   int32_t interpolation_radius, double center_easting, double center_northing,
-                                   uint32_t halo_capacity) {
-  if (!ctx) return AMB_ERR_INVALID_ARGUMENT;
-  if (!d_xyz || !d_ids) return AMB_ERR_INVALID_ARGUMENT;  // a sharded cloud needs global ids
-  if (interpolation_radius < 1) return AMB_ERR_INVALID_ARGUMENT;
-  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
-  if (ctx->comm_size <= 1 || !ctx->nccl_comm)  // not sharded: the whole cloud is here
-    return amb_dsm_process_device_ids(ctx, d_xyz, d_ids, n_local, interpolation_radius, center_easting,
-                                      center_northing);
-  return sharded_step(ctx, d_xyz, nullptr, d_ids, n_local, interpolation_radius, center_easting, center_northing,
-                      halo_capacity, 0);
-}
-
-int amb_ortho_from_pcl_process_sharded_device(amb_ctx* ctx, const double* d_xyz, const int32_t* d_intensities,
-                                              const uint64_t* d_ids, size_t n_local, int32_t interpolation_radius,
-                                              uint32_t halo_capacity) {
-  if (!ctx) return AMB_ERR_INVALID_ARGUMENT;
-  if (!d_xyz || !d_intensities || !d_ids) return AMB_ERR_INVALID_ARGUMENT;  // a sharded cloud needs global ids
-  if (interpolation_radius < 1) return AMB_ERR_INVALID_ARGUMENT;
-  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
-  if (ctx->comm_size <= 1 || !ctx->nccl_comm)  // not sharded: the whole cloud is here
-    return amb_ortho_from_pcl_process_device_ids(ctx, d_xyz, d_intensities, d_ids, n_local, interpolation_radius, 0);
-  return sharded_step(ctx, d_xyz, d_intensities, d_ids, n_local, interpolation_radius, 0.0, 0.0, halo_capacity, 1);
-}
-
-int amb_ortho_from_pcl_process_sharded(amb_ctx* ctx, const double* xyz, const int32_t* intensities, const uint64_t* ids,
-                                       size_t n_local, int32_t interpolation_radius, uint32_t halo_capacity) {
-  if (!ctx || !xyz || !intensities || !ids) return AMB_ERR_INVALID_ARGUMENT;
-  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
-  AMB_CUDA(ctx, ctx->points.reserve(std::max<size_t>(n_local, 1) * 3 * sizeof(double)));
-  AMB_CUDA(ctx, ctx->intensities.reserve(std::max<size_t>(n_local, 1) * sizeof(int32_t)));
-  AMB_CUDA(ctx, ctx->point_ids.reserve(std::max<size_t>(n_local, 1) * sizeof(uint64_t)));
-  if (n_local) {
-    const int sst = staged_h2d(ctx, ctx->points.ptr, xyz, n_local * 3 * sizeof(double), ctx->stream);
-    if (sst != AMB_OK) return sst;
-    AMB_CUDA(ctx, cudaMemcpyAsync(ctx->intensities.ptr, intensities, n_local * sizeof(int32_t), cudaMemcpyHostToDevice,
-                                  ctx->stream));
-    AMB_CUDA(ctx, cudaMemcpyAsync(ctx->point_ids.ptr, ids, n_local * sizeof(uint64_t), cudaMemcpyHostToDevice,
-                                  ctx->stream));
-  }
-  const int st = amb_ortho_from_pcl_process_sharded_device(ctx, ctx->points.as<double>(), ctx->intensities.as<int32_t>(),
-                                                           ctx->point_ids.as<uint64_t>(), n_local, interpolation_radius,
-                                                           halo_capacity);
-  if (st != AMB_OK) return st;
-  AMB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // host entry points are synchronous (ortho final on the device)
-  return AMB_OK;
-}
-
-int amb_dsm_process_sharded(amb_ctx* ctx, const double* xyz, const uint64_t* ids, size_t n_local,
-                            int32_t interpolation_radius, double center_easting, double center_northing,
-                            uint32_t halo_capacity) {
-  if (!ctx || !xyz || !ids) return AMB_ERR_INVALID_ARGUMENT;
-  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
-  AMB_CUDA(ctx, ctx->points.reserve(std::max<size_t>(n_local, 1) * 3 * sizeof(double)));
-  AMB_CUDA(ctx, ctx->point_ids.reserve(std::max<size_t>(n_local, 1) * sizeof(uint64_t)));
-  if (n_local) {
-    const int sst = staged_h2d(ctx, ctx->points.ptr, xyz, n_local * 3 * sizeof(double), ctx->stream);
-    if (sst != AMB_OK) return sst;
-    AMB_CUDA(ctx, cudaMemcpyAsync(ctx->point_ids.ptr, ids, n_local * sizeof(uint64_t), cudaMemcpyHostToDevice,
-                                  ctx->stream));
-  }
-  const int st = amb_dsm_process_sharded_device(ctx, ctx->points.as<double>(), ctx->point_ids.as<uint64_t>(), n_local,
-                                                interpolation_radius, center_easting, center_northing, halo_capacity);
-  if (st != AMB_OK) return st;
-  AMB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // host entry points are synchronous (elevation final on the device)
-  return AMB_OK;
-}
-
-}  // extern "C"

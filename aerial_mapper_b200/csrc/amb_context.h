@@ -282,6 +282,11 @@ int pcl_adaptive_finish(amb_ctx* ctx, int pass_status, const double* d_xyz, cons
                         const int* d_intensities, size_t n, int32_t interpolation_radius, float* saved);
 int ortho_run(amb_ctx* ctx, const amb_camera* camera, const double* T_G_B, const uint8_t* const* d_images,
               const uint8_t* const* h_images, size_t n, int32_t channels, size_t row_step, int32_t colored_ortho);
+// amb_comm.cu: one step of a sharded cloud on a context of a communicator of several ranks (halo exchange, then
+// dsm_run over the rank's points and the neighbours' halos); records the DSM events and sets dsm_timed itself
+int sharded_step(amb_ctx* ctx, const double* d_xyz, const int* d_intensities, const uint64_t* d_ids, size_t n_local,
+                 int32_t interpolation_radius, double center_easting, double center_northing, uint32_t halo_capacity,
+                 int mode);
 std::vector<double> dsm_thresholds(int32_t interpolation_radius);
 double dsm_tile_reach_cells(double resolution, int32_t interpolation_radius);  // tile width + window apron + 1, in cells
 

@@ -61,6 +61,21 @@ inline float* stripe_ptr(const amb_multi* m, int r, float* full) {
   return full + static_cast<size_t>(m->geom.rows) * static_cast<size_t>(m->ctx[r]->col_begin);
 }
 
+// One host cloud of n points to every stripe's host entry point process(ctx).  Bucket size / stage capacity — hence
+// every summation order — follow the density of the WHOLE cloud on every device; the adaptive OrthoFromPcl pass's
+// whole-map binning also needs it to visit the buckets of a single-GPU run.
+template <typename F>
+int cloud_to_every_stripe(amb_multi* m, size_t n, bool inputs, F process) {
+  if (!m) return AMB_ERR_INVALID_ARGUMENT;
+  if (n == 0) return AMB_ERR_EMPTY;  // dsm.cc:189-192, CHECK(!pointcloud.empty()) ortho-from-pcl.cc:23
+  if (!inputs) return AMB_ERR_INVALID_ARGUMENT;
+  const double per_cell = static_cast<double>(n) / (static_cast<double>(m->geom.rows) * static_cast<double>(m->geom.cols));
+  return for_each_stripe(m, [&](int, amb_ctx* c) {
+    const int st = amb_dsm_set_density_hint(c, per_cell);
+    return st == AMB_OK ? process(c) : st;
+  });
+}
+
 }  // namespace
 
 extern "C" {
@@ -156,31 +171,15 @@ int amb_multi_sync(amb_multi* m) {
 
 int amb_multi_dsm_process(amb_multi* m, const double* xyz, size_t n, int32_t interpolation_radius, double center_easting,
                           double center_northing) {
-  if (!m) return AMB_ERR_INVALID_ARGUMENT;
-  if (n == 0) return AMB_ERR_EMPTY;  // dsm.cc:189-192
-  if (!xyz) return AMB_ERR_INVALID_ARGUMENT;
-  // bucket size / stage capacity — hence every summation order — follow the density of the WHOLE cloud on every device
-  const double per_cell = static_cast<double>(n) / (static_cast<double>(m->geom.rows) * static_cast<double>(m->geom.cols));
-  return for_each_stripe(m, [&](int, amb_ctx* c) {
-    int st = amb_dsm_set_density_hint(c, per_cell);
-    if (st == AMB_OK) st = amb_dsm_process(c, xyz, n, interpolation_radius, center_easting, center_northing);
-    return st;
+  return cloud_to_every_stripe(m, n, xyz != nullptr, [&](amb_ctx* c) {
+    return amb_dsm_process(c, xyz, n, interpolation_radius, center_easting, center_northing);
   });
 }
 
 int amb_multi_ortho_from_pcl_process(amb_multi* m, const double* xyz, const int32_t* intensities, size_t n,
                                      int32_t interpolation_radius, int32_t use_adaptive_interpolation) {
-  if (!m) return AMB_ERR_INVALID_ARGUMENT;
-  if (n == 0) return AMB_ERR_EMPTY;  // CHECK(!pointcloud.empty()), ortho-from-pcl.cc:23
-  if (!xyz || !intensities) return AMB_ERR_INVALID_ARGUMENT;
-  // as amb_multi_dsm_process: the density of the WHOLE cloud fixes the bucket edge on every device, which the adaptive
-  // pass's whole-map binning also needs to visit the buckets of a single-GPU run
-  const double per_cell = static_cast<double>(n) / (static_cast<double>(m->geom.rows) * static_cast<double>(m->geom.cols));
-  return for_each_stripe(m, [&](int, amb_ctx* c) {
-    int st = amb_dsm_set_density_hint(c, per_cell);
-    if (st == AMB_OK)
-      st = amb_ortho_from_pcl_process(c, xyz, intensities, n, interpolation_radius, use_adaptive_interpolation);
-    return st;
+  return cloud_to_every_stripe(m, n, xyz && intensities, [&](amb_ctx* c) {
+    return amb_ortho_from_pcl_process(c, xyz, intensities, n, interpolation_radius, use_adaptive_interpolation);
   });
 }
 
