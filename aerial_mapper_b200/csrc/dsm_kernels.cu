@@ -272,8 +272,10 @@ __global__ void __launch_bounds__(256) dsm_mark_buckets_kernel(const __grid_cons
                                                                const unsigned int* __restrict__ cell_list,
                                                                const unsigned int* __restrict__ counters,
                                                                unsigned char* __restrict__ flags) {
-  const unsigned int n_cells = counters[CTR_DSM_LIST];
-  for (unsigned int c = blockIdx.x * blockDim.x + threadIdx.x; c < n_cells; c += gridDim.x * blockDim.x) {
+  // 64-bit cursor: a list can hold nearly 2^32 cells (amb_create), and a 32-bit c + stride would wrap past its end
+  const size_t n_cells = counters[CTR_DSM_LIST];
+  for (size_t c = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; c < n_cells;
+       c += static_cast<size_t>(gridDim.x) * blockDim.x) {
     const unsigned int cell = cell_list[c];
     const int i = static_cast<int>(cell % static_cast<unsigned int>(plan.rows));
     const int jl = static_cast<int>(cell / static_cast<unsigned int>(plan.rows));
@@ -518,9 +520,9 @@ struct CellArgs {
 
 __global__ void __launch_bounds__(256) dsm_cell_kernel(const __grid_constant__ DsmPlan plan, const CellArgs args) {
   const int lane = threadIdx.x & 31;
-  const unsigned int n_cells = args.counters[CTR_DSM_LIST];
-  const unsigned int warps_total = gridDim.x * (blockDim.x >> 5);
-  for (unsigned int c = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); c < n_cells; c += warps_total) {
+  const size_t n_cells = args.counters[CTR_DSM_LIST];
+  const size_t warps_total = static_cast<size_t>(gridDim.x) * (blockDim.x >> 5);  // 64-bit cursor, as above
+  for (size_t c = blockIdx.x * static_cast<size_t>(blockDim.x >> 5) + (threadIdx.x >> 5); c < n_cells; c += warps_total) {
     const unsigned int cell = args.cell_list[c];
     const int i = static_cast<int>(cell % static_cast<unsigned int>(plan.rows));
     const int jl = static_cast<int>(cell / static_cast<unsigned int>(plan.rows));

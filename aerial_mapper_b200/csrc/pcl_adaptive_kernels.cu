@@ -67,9 +67,9 @@ __global__ void __launch_bounds__(256) pcl_adaptive_list_kernel(const float* __r
 __global__ void __launch_bounds__(256) pcl_adaptive_cell_kernel(const __grid_constant__ DsmPlan plan,
                                                                 const __grid_constant__ AdaptiveArgs a) {
   const int lane = threadIdx.x & 31;
-  const unsigned int n_cells = *a.n_cells;
-  const unsigned int warps_total = gridDim.x * (blockDim.x >> 5);
-  for (unsigned int c = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); c < n_cells; c += warps_total) {
+  const size_t n_cells = *a.n_cells;
+  const size_t warps_total = static_cast<size_t>(gridDim.x) * (blockDim.x >> 5);  // 64-bit cursor: see dsm_cell_kernel
+  for (size_t c = blockIdx.x * static_cast<size_t>(blockDim.x >> 5) + (threadIdx.x >> 5); c < n_cells; c += warps_total) {
     const unsigned int cell = a.cell_list[c];
     const int i = static_cast<int>(cell % static_cast<unsigned int>(plan.rows));
     const int jl = static_cast<int>(cell / static_cast<unsigned int>(plan.rows));

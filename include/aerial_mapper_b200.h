@@ -132,7 +132,9 @@ int amb_geometry_position(const amb_geometry* geom, int32_t i, int32_t j, double
 
 /* ---- context ---- */
 /* Create a context on `device` owning columns [col_begin, col_end) of the map.  Pass 0, geom->cols for the
- * whole map.  Device layer slabs are allocated lazily (first upload / init / process that touches them). */
+ * whole map.  Device layer slabs are allocated lazily (first upload / init / process that touches them).
+ * Limits: a context holds fewer than 2^32 - 1 cells, rows * (col_end - col_begin) (else AMB_ERR_UNSUPPORTED), and the
+ * DSM and OrthoFromPcl take maps of fewer than 2^27 rows (else their process calls return AMB_ERR_UNSUPPORTED). */
 int amb_create(const amb_geometry* geom, int device, int32_t col_begin, int32_t col_end, amb_ctx** out);
 void amb_destroy(amb_ctx* ctx);
 int amb_sync(amb_ctx* ctx);
