@@ -82,80 +82,61 @@ static int nccl_fail(amb_ctx* ctx, int rc, const char* what) {
   return AMB_ERR_CUDA;
 }
 
-// Border halo of a sharded cloud as 32-byte records {x, y, z, id} behind a 32-byte header {count, ...}: exactly what the
-// binning kernels of every rank read after the all-gather.  Unordered append (warp-aggregated atomic): order does not
-// matter, every point carries its global id.
-// seg_up / seg_down: two segments (header + records).  A point near the stripe's LOW-column border (large y) goes to
-// seg_up — what the previous rank needs — one near the HIGH-column border to seg_down; with `split` = false everything
-// goes to seg_up (the all-gather exchange delivers one list per rank to everybody).
-__device__ __forceinline__ void halo_append(bool take, int lane, unsigned char* seg, unsigned int capacity, double x,
-                                            double y, double z, unsigned long long id) {
-  const unsigned int mask = __ballot_sync(0xffffffffu, take);
-  if (!mask) return;
-  const int leader = __ffs(mask) - 1;
-  unsigned int base = 0;
-  if (lane == leader) base = atomicAdd(reinterpret_cast<unsigned int*>(seg), static_cast<unsigned int>(__popc(mask)));
-  base = __shfl_sync(0xffffffffu, base, leader);
-  if (take) {
-    const unsigned int slot = base + __popc(mask & ((1u << lane) - 1u));
-    if (slot < capacity) {
-      double* r = reinterpret_cast<double*>(seg + 32) + 4 * static_cast<size_t>(slot);
-      r[0] = x;
-      r[1] = y;
-      r[2] = z;
-      r[3] = __longlong_as_double(static_cast<long long>(id));
-    }
-  }
-}
-
+// The border halo (halo_push.h) as segments of records, for the NCCL exchanges.  Unordered append: order does not matter,
+// every point carries its global id.  A point near the stripe's LOW-column border (large y) goes to seg_up — what the
+// previous rank needs — one near the HIGH-column border to seg_down; with `split` = false everything goes to seg_up
+// (the all-gather exchange delivers one list per rank to everybody).
 // INTENSITIES (OrthoFromPcl): the record's z is double(intensities[t]), what that pass bins (ortho-from-pcl.cc:33)
 template <bool INTENSITIES>
-__device__ __forceinline__ void halo_records(const double* __restrict__ xyz, const int* __restrict__ intensities,
-                                             const unsigned long long* __restrict__ ids, size_t n, double y_lo,
-                                             double y_hi, double reach, double shift_y, unsigned char* seg_up,
-                                             unsigned char* seg_down, bool split, unsigned int capacity) {
-  const int lane = threadIdx.x & 31;
+__global__ void __launch_bounds__(256) halo_records_kernel(const double* __restrict__ xyz,
+                                                           const int* __restrict__ intensities,
+                                                           const unsigned long long* __restrict__ ids, size_t n,
+                                                           double y_lo, double y_hi, double reach, double shift_y,
+                                                           unsigned char* seg_up, unsigned char* seg_down, bool split,
+                                                           unsigned int capacity) {
   const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
   const size_t n_round = ((n + stride - 1) / stride) * stride;  // whole warps stay converged for the ballots
   for (size_t t = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; t < n_round; t += stride) {
-    bool up = false, down = false;
+    BorderSides b = {false, false};
     double x = 0, y = 0, z = 0;
     unsigned long long id = 0;
     if (t < n) {
       y = xyz[3 * t + 1];
-      const double ys = y - shift_y;
-      up = ys > y_hi - reach;    // column 0 is the max-y side: the previous rank's stripe lies beyond y_hi
-      down = ys < y_lo + reach;
-      if (up || down) {
+      b = border_sides(y - shift_y, y_lo, y_hi, reach);
+      if (b.up || b.down) {
         x = xyz[3 * t + 0];
         z = INTENSITIES ? static_cast<double>(intensities[t]) : xyz[3 * t + 2];
         id = ids ? ids[t] : static_cast<unsigned long long>(t);
       }
     }
+    auto append = [&](bool take, unsigned char* seg) {
+      warp_reserve(take, halo_count(seg), [&](unsigned int slot) {
+        if (slot < capacity) store_record(halo_slot(seg, slot), x, y, z, id);
+      });
+    };
     if (split) {
-      halo_append(up, lane, seg_up, capacity, x, y, z, id);
-      halo_append(down, lane, seg_down, capacity, x, y, z, id);
+      append(b.up, seg_up);
+      append(b.down, seg_down);
     } else {
-      halo_append(up || down, lane, seg_up, capacity, x, y, z, id);
+      append(b.up || b.down, seg_up);
     }
   }
 }
 
-__global__ void __launch_bounds__(256) dsm_halo_records_kernel(const double* __restrict__ xyz,
-                                                               const unsigned long long* __restrict__ ids, size_t n,
-                                                               double y_lo, double y_hi, double reach, double shift_y,
-                                                               unsigned char* seg_up, unsigned char* seg_down, bool split,
-                                                               unsigned int capacity) {
-  halo_records<false>(xyz, nullptr, ids, n, y_lo, y_hi, reach, shift_y, seg_up, seg_down, split, capacity);
-}
-
-__global__ void __launch_bounds__(256) pcl_halo_records_kernel(const double* __restrict__ xyz,
-                                                               const int* __restrict__ intensities,
-                                                               const unsigned long long* __restrict__ ids, size_t n,
-                                                               double y_lo, double y_hi, double reach,
-                                                               unsigned char* seg_up, unsigned char* seg_down, bool split,
-                                                               unsigned int capacity) {
-  halo_records<true>(xyz, intensities, ids, n, y_lo, y_hi, reach, 0.0, seg_up, seg_down, split, capacity);
+int halo_compact(amb_ctx* ctx, const HaloCloud& c, unsigned char* seg_up, unsigned char* seg_down, bool split,
+                 unsigned int capacity) {
+  AMB_CUDA(ctx, cudaMemsetAsync(seg_up, 0, kHaloHeaderBytes, ctx->stream));
+  if (split) AMB_CUDA(ctx, cudaMemsetAsync(seg_down, 0, kHaloHeaderBytes, ctx->stream));
+  if (c.n == 0) return AMB_OK;
+  const int grid = ctx->num_sms * 8;
+  if (c.intensities)
+    halo_records_kernel<true><<<grid, 256, 0, ctx->stream>>>(c.xyz, c.intensities, c.ids, c.n, c.y_lo, c.y_hi, c.reach,
+                                                             c.shift_y, seg_up, seg_down, split, capacity);
+  else
+    halo_records_kernel<false><<<grid, 256, 0, ctx->stream>>>(c.xyz, nullptr, c.ids, c.n, c.y_lo, c.y_hi, c.reach,
+                                                              c.shift_y, seg_up, seg_down, split, capacity);
+  AMB_CUDA(ctx, cudaGetLastError());
+  return AMB_OK;
 }
 
 
@@ -245,7 +226,7 @@ static int peer_halo_setup(amb_ctx* ctx, uint32_t side_capacity) {
   }
   peer_halo_release(ctx);
   hp.tried = true;
-  const size_t side_bytes = 32 * (static_cast<size_t>(side_capacity) + 1);
+  const size_t side_bytes = halo_segment_bytes(side_capacity);
   PeerBlob mine;
   std::memset(&mine, 0, sizeof(mine));
   mine.pid = static_cast<long long>(getpid());
@@ -400,6 +381,79 @@ int amb_comm_rank(const amb_ctx* ctx) { return ctx ? ctx->comm_rank : -1; }
 
 namespace amb {
 
+// Exchange mode "all-gather": the rank's whole halo in one segment, and ONE ncclAllGather gives every rank every
+// rank's segment.
+static int exchange_all_gather(amb_ctx* ctx, const HaloCloud& c, uint32_t capacity, HaloSource* halo) {
+  const size_t seg_bytes = halo_segment_bytes(capacity);
+  AMB_CUDA(ctx, ctx->halo_send.reserve(seg_bytes));
+  AMB_CUDA(ctx, ctx->halo_recv.reserve(seg_bytes * ctx->comm_size));
+  unsigned char* send = ctx->halo_send.as<unsigned char>();
+  const int st = halo_compact(ctx, c, send, send, false, capacity);
+  if (st != AMB_OK) return st;
+  const int rc = nccl().all_gather(send, ctx->halo_recv.ptr, seg_bytes, kNcclInt8,
+                                   static_cast<nccl_comm_t>(ctx->nccl_comm), ctx->stream);
+  if (rc != 0) return nccl_fail(ctx, rc, "ncclAllGather");
+  ctx->halo_last_exchange = 1;
+  *halo = {ctx->halo_recv.as<unsigned char>(), ctx->comm_size, ctx->comm_rank, capacity, seg_bytes};
+  return AMB_OK;
+}
+
+// Exchange mode "send/recv": one segment per side, and two ncclSend / ncclRecv pairs in one group move each to the one
+// adjacent rank that needs it.  send: [up | down], recv: [from rank - 1 | from rank + 1].
+static int exchange_send_recv(amb_ctx* ctx, const HaloCloud& c, uint32_t side_capacity, HaloSource* halo) {
+  const int nranks = ctx->comm_size, rank = ctx->comm_rank;
+  const size_t side_bytes = halo_segment_bytes(side_capacity);
+  cudaStream_t s = ctx->stream;
+  AMB_CUDA(ctx, ctx->halo_send.reserve(2 * side_bytes));
+  AMB_CUDA(ctx, ctx->halo_recv.reserve(2 * side_bytes));
+  unsigned char* send = ctx->halo_send.as<unsigned char>();
+  unsigned char* recv = ctx->halo_recv.as<unsigned char>();
+  AMB_CUDA(ctx, cudaMemsetAsync(recv, 0, kHaloHeaderBytes, s));  // a missing neighbour contributes an empty list
+  AMB_CUDA(ctx, cudaMemsetAsync(recv + side_bytes, 0, kHaloHeaderBytes, s));
+  const int st = halo_compact(ctx, c, send, send + side_bytes, true, side_capacity);
+  if (st != AMB_OK) return st;
+  nccl_comm_t comm = static_cast<nccl_comm_t>(ctx->nccl_comm);
+  int rc = nccl().group_start();
+  if (rc == 0 && rank > 0) rc = nccl().send(send, side_bytes, kNcclInt8, rank - 1, comm, s);
+  if (rc == 0 && rank > 0) rc = nccl().recv(recv, side_bytes, kNcclInt8, rank - 1, comm, s);
+  if (rc == 0 && rank < nranks - 1) rc = nccl().send(send + side_bytes, side_bytes, kNcclInt8, rank + 1, comm, s);
+  if (rc == 0 && rank < nranks - 1) rc = nccl().recv(recv + side_bytes, side_bytes, kNcclInt8, rank + 1, comm, s);
+  const int rc_end = nccl().group_end();
+  if (rc != 0 || rc_end != 0) return nccl_fail(ctx, rc != 0 ? rc : rc_end, "ncclSend/ncclRecv (halo)");
+  ctx->halo_last_exchange = 2;
+  *halo = {recv, 2, -1, side_capacity, side_bytes};  // both segments are foreign
+  return AMB_OK;
+}
+
+// Exchange mode "peer push": the partition kernel of the binning (dsm_run) stores the border records into the
+// neighbours' segments of this step's parity while it bins the rank's own points and publishes the counts;
+// halo_wait_kernel then holds the binning of the incoming halos back until both neighbours have published theirs.
+static void exchange_peer_push(amb_ctx* ctx, const HaloCloud& c, uint32_t side_capacity, HaloSource* halo,
+                               HaloPush* push) {
+  HaloPeer& hp = ctx->halo_peer;
+  const int nranks = ctx->comm_size, rank = ctx->comm_rank;
+  const size_t peer_side_bytes = halo_segment_bytes(hp.side_capacity);
+  const unsigned int parity = static_cast<unsigned int>(hp.step & 1u);
+  const unsigned int stamp = static_cast<unsigned int>(hp.step + 1);
+  ++hp.step;
+  // segment layout of every rank: [parity][0 = filled by rank - 1 | 1 = filled by rank + 1]
+  push->seg_up = hp.prev ? hp.prev + (2 * parity + 1) * peer_side_bytes : nullptr;    // I am rank - 1's "rank + 1"
+  push->seg_down = hp.next ? hp.next + (2 * parity + 0) * peer_side_bytes : nullptr;  // I am rank + 1's "rank - 1"
+  push->counters = hp.counters + 4 * parity;
+  push->capacity = side_capacity;
+  push->stamp = stamp;
+  push->y_lo = c.y_lo;
+  push->y_hi = c.y_hi;
+  push->reach = c.reach;
+  push->shift_y = c.shift_y;
+  unsigned char* mine = hp.recv + 2 * parity * peer_side_bytes;
+  push->wait_prev = rank > 0 ? mine : nullptr;
+  push->wait_next = rank < nranks - 1 ? mine + peer_side_bytes : nullptr;
+  ctx->halo_last_exchange = 4;
+  // both segments are foreign (a missing neighbour's header stays {0, 0}: an empty list)
+  *halo = {mine, 2, -1, side_capacity, peer_side_bytes};
+}
+
 // The sharded step shared by Dsm (mode 0) and OrthoFromPcl (mode 1, d_intensities: every record's z is the point's
 // intensity, no centre shift): exchange of the border halos, then the binning over [own points | neighbours' halos].
 // The caller has checked the arguments and that the context belongs to a communicator of several ranks.
@@ -407,34 +461,25 @@ int sharded_step(amb_ctx* ctx, const double* d_xyz, const int* d_intensities, co
                  size_t n_local, int32_t interpolation_radius, double center_easting, double center_northing,
                  uint32_t halo_capacity, int mode) {
   if (halo_capacity == 0) return AMB_ERR_INVALID_ARGUMENT;
-  const int nranks = ctx->comm_size, rank = ctx->comm_rank;
-  const size_t seg_bytes = 32 * (static_cast<size_t>(halo_capacity) + 1);  // header + records
-  cudaStream_t s = ctx->stream;
-  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_BEGIN], s));
-  double y_lo = 0, y_hi = 0;
-  int st = amb_stripe_y_interval(&ctx->geom, ctx->col_begin, ctx->col_end, &y_lo, &y_hi);
+  const int nranks = ctx->comm_size;
+  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_BEGIN], ctx->stream));
+  HaloCloud c;
+  c.xyz = d_xyz;
+  c.intensities = d_intensities;
+  c.ids = reinterpret_cast<const unsigned long long*>(d_ids);
+  c.n = n_local;
+  int st = amb_stripe_y_interval(&ctx->geom, ctx->col_begin, ctx->col_end, &c.y_lo, &c.y_hi);
   if (st != AMB_OK) return st;
-  const double reach = amb_dsm_halo_reach(&ctx->geom, interpolation_radius);
-  // compaction of this rank's border points into exchange segments (the NCCL exchanges; peer push compacts in the binning)
-  auto compact = [&](unsigned char* seg_up, unsigned char* seg_down, bool split, uint32_t capacity) {
-    if (n_local == 0) return cudaSuccess;
-    const unsigned long long* ids = reinterpret_cast<const unsigned long long*>(d_ids);
-    if (d_intensities)
-      pcl_halo_records_kernel<<<ctx->num_sms * 8, 256, 0, s>>>(d_xyz, d_intensities, ids, n_local, y_lo, y_hi, reach,
-                                                               seg_up, seg_down, split, capacity);
-    else
-      dsm_halo_records_kernel<<<ctx->num_sms * 8, 256, 0, s>>>(d_xyz, ids, n_local, y_lo, y_hi, reach, center_easting,
-                                                               seg_up, seg_down, split, capacity);
-    return cudaGetLastError();
-  };
+  c.reach = amb_dsm_halo_reach(&ctx->geom, interpolation_radius);
+  c.shift_y = d_intensities ? 0.0 : center_easting;
 
   // Who needs this rank's border points?  If the stripes are consecutive (rank r + 1 starts where rank r ends) and every
-  // stripe is at least `reach` wide, only the two adjacent ranks do: two ncclSend / ncclRecv pairs in one group move each
-  // half of the halo to the one rank that stages it.  Otherwise (narrow or irregular stripes) ONE ncclAllGather gives
+  // stripe is at least `reach` wide, only the two adjacent ranks do: each half of the halo goes to the one rank that
+  // stages it (peer push, or ncclSend / ncclRecv).  Otherwise (narrow or irregular stripes) ONE ncclAllGather gives
   // every rank every halo.  The decision uses the stripes gathered at amb_comm_init: identical on all ranks.
   bool neighbours = ctx->halo_exchange_mode != 1;
   if (ctx->halo_exchange_mode == 0 || ctx->halo_exchange_mode == 3) {
-    const double reach_cols = reach / ctx->geom.resolution;
+    const double reach_cols = c.reach / ctx->geom.resolution;
     for (int r = 0; r < nranks && neighbours; ++r) {
       const int32_t b = ctx->comm_stripes[2 * r], e = ctx->comm_stripes[2 * r + 1];
       if (static_cast<double>(e - b) < reach_cols + 1.0) neighbours = false;
@@ -444,14 +489,8 @@ int sharded_step(amb_ctx* ctx, const double* d_xyz, const int* d_intensities, co
   HaloSource halo;
   HaloPush push;
   bool use_push = false;
-  halo.capacity = halo_capacity;
-  halo.seg_bytes = seg_bytes;
   if (neighbours) {
-    // each list holds ONE side of the halo: half the capacity
-    const uint32_t side_capacity = halo_capacity / 2 + 1;
-    const size_t side_bytes = 32 * (static_cast<size_t>(side_capacity) + 1);
-    halo.capacity = side_capacity;
-    halo.seg_bytes = side_bytes;
+    const uint32_t side_capacity = halo_capacity / 2 + 1;  // each list holds ONE side of the halo: half the capacity
     HaloPeer& hp = ctx->halo_peer;
     if (!hp.tried) {
       const char* e = std::getenv("AMB_HALO_PEER");  // development switch: AMB_HALO_PEER=0 keeps ncclSend/ncclRecv
@@ -463,76 +502,19 @@ int sharded_step(amb_ctx* ctx, const double* d_xyz, const int* d_intensities, co
       st = peer_halo_setup(ctx, side_capacity);
       if (st != AMB_OK) return st;
     }
-    if (hp.enabled && ctx->halo_exchange_mode != 3) {
-      // peer push: the partition kernel of the binning (dsm_run) stores the border records into the neighbours' segments of
-      // this step's parity while it bins the rank's own points and publishes the counts; halo_wait_kernel then holds the
-      // binning of the incoming halos back until both neighbours have published theirs
-      const size_t peer_side_bytes = 32 * (static_cast<size_t>(hp.side_capacity) + 1);
-      const unsigned int parity = static_cast<unsigned int>(hp.step & 1u);
-      const unsigned int stamp = static_cast<unsigned int>(hp.step + 1);
-      ++hp.step;
-      // segment layout of every rank: [parity][0 = filled by rank - 1 | 1 = filled by rank + 1]
-      push.seg_up = hp.prev ? hp.prev + (2 * parity + 1) * peer_side_bytes : nullptr;    // I am rank - 1's "rank + 1"
-      push.seg_down = hp.next ? hp.next + (2 * parity + 0) * peer_side_bytes : nullptr;  // I am rank + 1's "rank - 1"
-      push.counters = hp.counters + 4 * parity;
-      push.capacity = side_capacity;
-      push.stamp = stamp;
-      push.y_lo = y_lo;
-      push.y_hi = y_hi;
-      push.reach = reach;
-      push.shift_y = center_easting;
-      unsigned char* mine = hp.recv + 2 * parity * peer_side_bytes;
-      push.wait_prev = rank > 0 ? mine : nullptr;
-      push.wait_next = rank < nranks - 1 ? mine + peer_side_bytes : nullptr;
-      use_push = true;
-      ctx->halo_last_exchange = 4;
-      halo.gathered = mine;
-      halo.seg_bytes = peer_side_bytes;
-      halo.nranks = 2;
-      halo.my_rank = -1;  // both segments are foreign (a missing neighbour's header stays {0, 0}: an empty list)
-    } else {
-    // send: [up | down], recv: [from rank - 1 | from rank + 1]
-    AMB_CUDA(ctx, ctx->halo_send.reserve(2 * side_bytes));
-    AMB_CUDA(ctx, ctx->halo_recv.reserve(2 * side_bytes));
-    unsigned char* send = ctx->halo_send.as<unsigned char>();
-    unsigned char* recv = ctx->halo_recv.as<unsigned char>();
-    AMB_CUDA(ctx, cudaMemsetAsync(send, 0, 32, s));
-    AMB_CUDA(ctx, cudaMemsetAsync(send + side_bytes, 0, 32, s));
-    AMB_CUDA(ctx, cudaMemsetAsync(recv, 0, 32, s));              // a missing neighbour contributes an empty list
-    AMB_CUDA(ctx, cudaMemsetAsync(recv + side_bytes, 0, 32, s));
-    AMB_CUDA(ctx, compact(send, send + side_bytes, true, side_capacity));
-    nccl_comm_t comm = static_cast<nccl_comm_t>(ctx->nccl_comm);
-    int rc = nccl().group_start();
-    if (rc == 0 && rank > 0) rc = nccl().send(send, side_bytes, kNcclInt8, rank - 1, comm, s);
-    if (rc == 0 && rank > 0) rc = nccl().recv(recv, side_bytes, kNcclInt8, rank - 1, comm, s);
-    if (rc == 0 && rank < nranks - 1) rc = nccl().send(send + side_bytes, side_bytes, kNcclInt8, rank + 1, comm, s);
-    if (rc == 0 && rank < nranks - 1) rc = nccl().recv(recv + side_bytes, side_bytes, kNcclInt8, rank + 1, comm, s);
-    const int rc_end = nccl().group_end();
-    if (rc != 0 || rc_end != 0) return nccl_fail(ctx, rc != 0 ? rc : rc_end, "ncclSend/ncclRecv (halo)");
-    ctx->halo_last_exchange = 2;
-    halo.gathered = recv;
-    halo.nranks = 2;
-    halo.my_rank = -1;  // both segments are foreign
-    }
+    use_push = hp.enabled && ctx->halo_exchange_mode != 3;
+    if (use_push)
+      exchange_peer_push(ctx, c, side_capacity, &halo, &push);
+    else
+      st = exchange_send_recv(ctx, c, side_capacity, &halo);
   } else {
-    AMB_CUDA(ctx, ctx->halo_send.reserve(seg_bytes));
-    AMB_CUDA(ctx, ctx->halo_recv.reserve(seg_bytes * nranks));
-    unsigned char* send = ctx->halo_send.as<unsigned char>();
-    AMB_CUDA(ctx, cudaMemsetAsync(send, 0, 32, s));
-    AMB_CUDA(ctx, compact(send, send, false, halo_capacity));
-    // the one collective of the step
-    const int rc = nccl().all_gather(send, ctx->halo_recv.ptr, seg_bytes, kNcclInt8,
-                                     static_cast<nccl_comm_t>(ctx->nccl_comm), s);
-    if (rc != 0) return nccl_fail(ctx, rc, "ncclAllGather");
-    ctx->halo_last_exchange = 1;
-    halo.gathered = ctx->halo_recv.as<unsigned char>();
-    halo.nranks = nranks;
-    halo.my_rank = rank;
+    st = exchange_all_gather(ctx, c, halo_capacity, &halo);
   }
-  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_H2D_END], s));  // "h2d" slot of the timings = the halo step
+  if (st != AMB_OK) return st;
+  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_H2D_END], ctx->stream));  // "h2d" slot of the timings = the halo step
   ctx->dsm_had_h2d = true;
-  st = dsm_run(ctx, d_xyz, reinterpret_cast<const unsigned long long*>(d_ids), n_local, interpolation_radius,
-               center_easting, center_northing, mode, d_intensities, &halo, use_push ? &push : nullptr);
+  st = dsm_run(ctx, d_xyz, c.ids, n_local, interpolation_radius, center_easting, center_northing, mode, d_intensities,
+               &halo, use_push ? &push : nullptr);
   ctx->dsm_timed = (st == AMB_OK);
   return st;
 }

@@ -116,14 +116,11 @@ struct CompactMirror {
   std::atomic<int> jobs_in_flight{0}; // chunks of the current round still being widened by the expander pool
 };
 
-// The neighbours' border halos as delivered by the all-gather (amb_comm.cu): nranks segments of seg_bytes, each a 32-byte
-// header {uint32 count, ...} followed by `capacity` 32-byte records {x, y, z, id}.  The binning kernels read them
-// after the rank's own points; the segment of the rank itself is skipped (those points are already local).
-// Peer-push halo exchange (amb_comm.cu): this rank's receive segments [parity 0/1][from rank - 1 | from rank + 1] and the
-// mapped pointers to the two neighbours' segments.
+// Peer-push halo exchange (amb_comm.cu, halo_push.h): this rank's receive segments [parity 0/1][from rank - 1 | from
+// rank + 1] and the mapped pointers to the two neighbours' segments.
 struct HaloPeer {
   bool enabled = false, tried = false, disabled = false;
-  unsigned char* recv = nullptr;       // own, cudaMalloc: 4 segments of 32 * (side_capacity + 1) bytes
+  unsigned char* recv = nullptr;       // own, cudaMalloc: 4 segments of halo_segment_bytes(side_capacity)
   unsigned int* counters = nullptr;    // own: [parity][up count, down count, blocks done, -]
   unsigned char* prev = nullptr;       // rank - 1's `recv`, mapped (cudaIpcOpenMemHandle or same-process peer access)
   unsigned char* next = nullptr;
@@ -131,13 +128,6 @@ struct HaloPeer {
   uint32_t side_capacity = 0, tried_capacity = 0;
   uint64_t step = 0;
   std::vector<unsigned char*> retired;   // segments replaced by a larger re-setup: freed when the communicator is left
-};
-
-struct HaloSource {
-  const unsigned char* gathered = nullptr;
-  int nranks = 0, my_rank = 0;
-  unsigned int capacity = 0;
-  size_t seg_bytes = 0;
 };
 
 }  // namespace amb
@@ -226,7 +216,8 @@ struct amb_ctx {
 
 namespace amb {
 
-struct HaloPush;  // halo_push.h
+struct HaloSource;  // halo_push.h
+struct HaloPush;
 
 inline int fail(amb_ctx* ctx, cudaError_t e, const char* what) {
   if (ctx) {

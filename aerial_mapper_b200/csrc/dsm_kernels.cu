@@ -68,30 +68,6 @@ constexpr int kScanChunk = 4096;    // elements per block in the scan kernels (2
 constexpr int kSortRegs = 4;        // bucket sort: records per lane held in registers (buckets up to 128 points)
 static_assert(TJ == kStrip * (kGatherThreads / 32), "one warp per strip row of the tile");
 
-// One 32-byte record = two 128-bit accesses (sm_90's widest: STG.E.128 / LDG.E.128) = exactly one DRAM sector.
-__device__ __forceinline__ void store_rec(PointRec* dst, double x, double y, double z, unsigned long long idx) {
-#ifdef AMB_CUDA_EMU  // tests/emu (CPU emulation of the kernel source)
-  dst->x = x;
-  dst->y = y;
-  dst->z = z;
-  dst->idx = idx;
-#else
-  asm volatile("st.global.v2.f64 [%0], {%1, %2};\n\tst.global.v2.f64 [%0+16], {%3, %4};" ::"l"(dst), "d"(x), "d"(y),
-               "d"(z), "d"(__longlong_as_double(static_cast<long long>(idx)))
-               : "memory");
-#endif
-}
-// Slot `s` of the gathered halos -> its record, or nullptr (own segment, beyond the segment's count).
-__device__ __forceinline__ const double* halo_record(const HaloSource& h, size_t s) {
-  const unsigned int r = static_cast<unsigned int>(s / h.capacity);
-  const unsigned int k = static_cast<unsigned int>(s - static_cast<size_t>(r) * h.capacity);
-  if (static_cast<int>(r) == h.my_rank) return nullptr;
-  const unsigned char* seg = h.gathered + static_cast<size_t>(r) * h.seg_bytes;
-  if (k >= *reinterpret_cast<const unsigned int*>(seg)) return nullptr;
-  return reinterpret_cast<const double*>(seg + 32) + 4 * static_cast<size_t>(k);
-}
-
-
 // ---------------------------------------------------------------------------------------------------------------
 // K2: inclusive scan (reduce / spine / apply).
 __device__ __forceinline__ unsigned int block_exclusive_scan(unsigned int v, unsigned int* total) {
@@ -650,18 +626,16 @@ inline int round_up(int v, int m) { return ((v + m - 1) / m) * m; }
 
 }  // namespace
 
-// Points of a sharded cloud that lie within `reach` of the borders of the y-interval (y_lo, y_hi] a rank owns:
-// what its neighbours need for interpolation (the "border halo").  Unordered append (warp-aggregated atomic);
-// order does not matter because every point carries its global id.
-// INTENSITIES (OrthoFromPcl): each point's intensity travels beside its coordinates.
+// The border halo (halo_push.h) of a sharded cloud as separate arrays: coordinates, intensities (INTENSITIES, OrthoFromPcl)
+// and ids.  Unordered append; order does not matter because every point carries its global id.
 template <bool INTENSITIES>
-__device__ __forceinline__ void halo_compact(const double* __restrict__ xyz, const int* __restrict__ intensities,
-                                             const unsigned long long* __restrict__ ids, size_t n, double y_lo,
-                                             double y_hi, double reach, double shift_y, double* __restrict__ out_xyz,
-                                             int* __restrict__ out_intensities,
-                                             unsigned long long* __restrict__ out_ids, unsigned int capacity,
-                                             unsigned int* __restrict__ count) {
-  const int lane = threadIdx.x & 31;
+__global__ void __launch_bounds__(256) halo_compact_kernel(const double* __restrict__ xyz,
+                                                           const int* __restrict__ intensities,
+                                                           const unsigned long long* __restrict__ ids, size_t n,
+                                                           double y_lo, double y_hi, double reach, double shift_y,
+                                                           double* __restrict__ out_xyz, int* __restrict__ out_intensities,
+                                                           unsigned long long* __restrict__ out_ids,
+                                                           unsigned int capacity, unsigned int* __restrict__ count) {
   const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
   const size_t n_round = ((n + stride - 1) / stride) * stride;  // whole warps stay converged for the ballot
   for (size_t t = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; t < n_round; t += stride) {
@@ -673,47 +647,18 @@ __device__ __forceinline__ void halo_compact(const double* __restrict__ xyz, con
       y = xyz[3 * t + 1];
       z = xyz[3 * t + 2];
       if (INTENSITIES) v = intensities[t];
-      const double ys = y - shift_y;
-      take = (ys < y_lo + reach) || (ys > y_hi - reach);
+      const BorderSides b = border_sides(y - shift_y, y_lo, y_hi, reach);
+      take = b.up || b.down;
     }
-    const unsigned int mask = __ballot_sync(0xffffffffu, take);
-    if (mask) {
-      const int leader = __ffs(mask) - 1;
-      unsigned int base = 0;
-      if (lane == leader) base = atomicAdd(count, static_cast<unsigned int>(__popc(mask)));
-      base = __shfl_sync(0xffffffffu, base, leader);
-      if (take) {
-        const unsigned int slot = base + __popc(mask & ((1u << lane) - 1u));
-        if (slot < capacity) {
-          out_xyz[3 * static_cast<size_t>(slot) + 0] = x;
-          out_xyz[3 * static_cast<size_t>(slot) + 1] = y;
-          out_xyz[3 * static_cast<size_t>(slot) + 2] = z;
-          if (INTENSITIES) out_intensities[slot] = v;
-          out_ids[slot] = ids ? ids[t] : static_cast<unsigned long long>(t);
-        }
-      }
-    }
+    warp_reserve(take, count, [&](unsigned int slot) {
+      if (slot >= capacity) return;
+      out_xyz[3 * static_cast<size_t>(slot) + 0] = x;
+      out_xyz[3 * static_cast<size_t>(slot) + 1] = y;
+      out_xyz[3 * static_cast<size_t>(slot) + 2] = z;
+      if (INTENSITIES) out_intensities[slot] = v;
+      out_ids[slot] = ids ? ids[t] : static_cast<unsigned long long>(t);
+    });
   }
-}
-
-__global__ void __launch_bounds__(256) dsm_halo_kernel(const double* __restrict__ xyz,
-                                                       const unsigned long long* __restrict__ ids, size_t n,
-                                                       double y_lo, double y_hi, double reach, double shift_y,
-                                                       double* __restrict__ out_xyz,
-                                                       unsigned long long* __restrict__ out_ids,
-                                                       unsigned int capacity, unsigned int* __restrict__ count) {
-  halo_compact<false>(xyz, nullptr, ids, n, y_lo, y_hi, reach, shift_y, out_xyz, nullptr, out_ids, capacity, count);
-}
-
-__global__ void __launch_bounds__(256) pcl_halo_kernel(const double* __restrict__ xyz,
-                                                       const int* __restrict__ intensities,
-                                                       const unsigned long long* __restrict__ ids, size_t n,
-                                                       double y_lo, double y_hi, double reach,
-                                                       double* __restrict__ out_xyz, int* __restrict__ out_intensities,
-                                                       unsigned long long* __restrict__ out_ids,
-                                                       unsigned int capacity, unsigned int* __restrict__ count) {
-  halo_compact<true>(xyz, intensities, ids, n, y_lo, y_hi, reach, 0.0, out_xyz, out_intensities, out_ids, capacity,
-                     count);
 }
 
 int dsm_extract_halo(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, size_t n, double y_lo,
@@ -722,12 +667,13 @@ int dsm_extract_halo(amb_ctx* ctx, const double* d_xyz, const unsigned long long
                      const int* d_intensities, int* d_out_intensities) {
   AMB_CUDA(ctx, cudaMemsetAsync(d_count, 0, sizeof(unsigned int), ctx->stream));
   if (d_intensities)  // OrthoFromPcl: no centre shift (ortho-from-pcl.cc bins the raw coordinates)
-    pcl_halo_kernel<<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(d_xyz, d_intensities, d_ids, n, y_lo, y_hi, reach,
-                                                               d_out_xyz, d_out_intensities, d_out_ids, capacity,
-                                                               d_count);
+    halo_compact_kernel<true><<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(d_xyz, d_intensities, d_ids, n, y_lo, y_hi,
+                                                                          reach, 0.0, d_out_xyz, d_out_intensities,
+                                                                          d_out_ids, capacity, d_count);
   else
-    dsm_halo_kernel<<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(d_xyz, d_ids, n, y_lo, y_hi, reach, center_easting,
-                                                               d_out_xyz, d_out_ids, capacity, d_count);
+    halo_compact_kernel<false><<<ctx->num_sms * 8, 256, 0, ctx->stream>>>(d_xyz, nullptr, d_ids, n, y_lo, y_hi, reach,
+                                                                           center_easting, d_out_xyz, nullptr,
+                                                                           d_out_ids, capacity, d_count);
   AMB_CUDA(ctx, cudaGetLastError());
   return AMB_OK;
 }

@@ -8,6 +8,8 @@
 
 #include <cfloat>
 #include <cstddef>
+
+#include "halo_push.h"
 namespace amb {
 namespace dsmk {
 
@@ -105,18 +107,10 @@ __device__ __forceinline__ double window_min_d2(const DsmPlan& p, const unsigned
   return dmin;
 }
 
-// Warp-aggregated append: every lane of the warp calls it; the lanes with `take` store `value` to consecutive slots of
-// `list` in lane order, reserved by one atomic on `*counter`.
+// Warp-aggregated append (every lane of the warp calls it): the lanes with `take` store `value` to consecutive slots
+// of `list` in lane order.
 __device__ __forceinline__ void warp_append(bool take, unsigned int* counter, unsigned int* list, unsigned int value) {
-  const unsigned int mask = __ballot_sync(0xffffffffu, take);
-  if (mask) {
-    const int lane = threadIdx.x & 31;
-    const int leader = __ffs(mask) - 1;
-    unsigned int base = 0;
-    if (lane == leader) base = atomicAdd(counter, static_cast<unsigned int>(__popc(mask)));
-    base = __shfl_sync(0xffffffffu, base, leader);
-    if (take) list[base + __popc(mask & ((1u << lane) - 1u))] = value;
-  }
+  warp_reserve(take, counter, [&](unsigned int slot) { list[slot] = value; });
 }
 
 // Reciprocal of a positive normal double to ~1 ulp: MUFU.RCP64H seed (rcp.approx.ftz.f64) + one cubic correction
