@@ -257,6 +257,35 @@ class GridMap(object):
         return _jpeg_call(lambda buf, cap, size: lib().amb_export_jpeg(ctx, LAYER_ID[name], f, *args[3:], buf, cap, size),
                           args, ctx)
 
+    def to_geotiff(self, path, name, fmt=None, epsg=32632, nodata=None, rows_per_strip=None):
+        """Writes the context's band of layer `name` to `path` as a Deflate-compressed GeoTIFF, predicted and compressed
+        on the device (convention: include/aerial_mapper_b200.h, amb_deflate_strips_device); reading it back gives
+        to_raster(name, fmt) bit for bit.  fmt: "f32", "gray8", "bgr8" or "mask8"; by default "f32" for `elevation`,
+        "gray8" for `ortho` and "bgr8" for `colored_ortho`, required for any other layer.  The geotransform is the
+        band's own: a stripe context writes its rows of the map as a file of their own.  nodata: GDAL_NODATA, e.g.
+        "nan".  rows_per_strip: by default libtiff's 8 KiB strips, max(1, 8192 // row_bytes)."""
+        if not self._resident:
+            raise AmbError(_lib.AMB_ERR_INVALID_ARGUMENT,
+                           "to_geotiff exports device-resident layers: call to_device() first")
+        if fmt is None:
+            fmt = {"elevation": "f32", "ortho": "gray8", "colored_ortho": "bgr8"}.get(name)
+            if fmt is None:
+                raise ValueError("to_geotiff(%r): give fmt='f32', 'gray8', 'bgr8' or 'mask8' for this layer" % (name,))
+        if fmt not in _lib.RASTER_FORMAT:
+            raise ValueError("to_geotiff: fmt must be 'f32', 'gray8', 'bgr8' or 'mask8', got %r" % (fmt,))
+        f = _lib.RASTER_FORMAT[fmt]
+        c0, c1 = self._col_range
+        width, height = self.geometry.rows, c1 - c0
+        rps = _deflate_rows(width * _lib.RASTER_BPP[f], height, rows_per_strip)
+        ctx = self._ctx
+        data, counts = _deflate_call(
+            lambda buf, cap, size, sb: lib().amb_export_deflate_strips(ctx, LAYER_ID[name], f, rps, buf, cap, size, sb),
+            width, height, f, rps, ctx)
+        gt = list(self.geotransform())
+        gt[3] += c0 * gt[5]        # the band's north edge
+        from . import io
+        io.write_geotiff_strips(path, data, counts, width, height, fmt, rps, gt, epsg, nodata)
+
     def timings(self):
         t = _lib.Timings()
         check(lib().amb_get_timings(self.context(), C.byref(t)), self._ctx)
@@ -703,7 +732,8 @@ _jpeg_contexts = {}
 
 
 def _jpeg_context(device):
-    """A context per device for encode_jpeg: only its stream and its scratch are used (a 1 x 1 map, no layers)."""
+    """A context per device for encode_jpeg and deflate_strips: only its stream and its scratch are used (a 1 x 1 map,
+    no layers)."""
     ctx = _jpeg_contexts.get(device)
     if ctx is None:
         g = Geometry()
@@ -739,3 +769,63 @@ def encode_jpeg(image, quality=95, sampling="420", restart_interval=0):
     return _jpeg_call(lambda buf, cap, size: lib().amb_jpeg_encode_device(ctx, C.c_void_p(image.data_ptr()), args[0],
                                                                           args[1], stride, *args[2:], buf, cap, size),
                       args, ctx)
+
+
+# ---- Deflate strips of a GeoTIFF (amb_deflate_strips_device, amb_export_deflate_strips) -------------------------------
+def _deflate_rows(row_bytes, height, rows_per_strip):
+    """rows_per_strip, by default libtiff's 8 KiB strip max(1, 8192 // row_bytes), capped at the height."""
+    if rows_per_strip is None:
+        return max(1, min(height, 8192 // row_bytes))
+    if isinstance(rows_per_strip, bool) or not isinstance(rows_per_strip, (int, np.integer)) or rows_per_strip < 1:
+        raise ValueError("rows_per_strip must be a positive integer, got %r" % (rows_per_strip,))
+    return int(min(rows_per_strip, height, 0x7FFFFFFF))
+
+
+def _deflate_call(call, width, height, fmt, rps, ctx):
+    """Runs `call(buffer, capacity, size, strip_bytes)` with a buffer of amb_deflate_max_size bytes; returns the strips
+    (bytes) and their lengths (uint32 array)."""
+    cap = lib().amb_deflate_max_size(width, height, fmt, rps)
+    if cap == 0:
+        raise AmbError(_lib.AMB_ERR_UNSUPPORTED, "a %d x %d raster in strips of %d rows" % (width, height, rps))
+    buf = np.empty(cap, np.uint8)
+    counts = np.zeros((height + rps - 1) // rps, np.uint32)
+    size = C.c_size_t(0)
+    check(call(buf.ctypes.data_as(C.c_void_p), cap, C.byref(size), counts.ctypes.data_as(C.c_void_p)), ctx)
+    return buf[:size.value].tobytes(), counts
+
+
+_DEFLATE_DTYPES = {"f32": "float32", "gray8": "uint8", "mask8": "uint8", "bgr8": "uint8"}
+
+
+def deflate_strips(image, fmt, rows_per_strip=None):
+    """The Deflate-compressed GeoTIFF strips of a torch CUDA raster, compressed on its device (convention:
+    include/aerial_mapper_b200.h, amb_deflate_strips_device): returns (strips as bytes, uint32 length of each strip,
+    rows_per_strip), ready for io.write_geotiff_strips.  image: float32 H x W for fmt "f32", uint8 H x W for "gray8" and
+    "mask8", uint8 H x W x 3 (B, G, R) for "bgr8".  Rows may be padded (a row-sliced view), pixels must be packed.  Waits
+    for the work queued on the current torch stream before reading the image."""
+    import torch
+    if fmt not in _DEFLATE_DTYPES:
+        raise ValueError("deflate_strips: fmt must be 'f32', 'gray8', 'bgr8' or 'mask8', got %r" % (fmt,))
+    if not isinstance(image, torch.Tensor) or not image.is_cuda or \
+            image.dtype != getattr(torch, _DEFLATE_DTYPES[fmt]):
+        raise ValueError("deflate_strips: expected a torch CUDA %s tensor for %r" % (_DEFLATE_DTYPES[fmt], fmt))
+    channels = 3 if fmt == "bgr8" else 1
+    if image.dim() != (3 if channels == 3 else 2) or (channels == 3 and image.shape[2] != 3):
+        raise ValueError("deflate_strips: expected %s for %r, got %s"
+                         % ("H x W x 3" if channels == 3 else "H x W", fmt, tuple(image.shape)))
+    h, w = int(image.shape[0]), int(image.shape[1])
+    inner = (1,) if channels == 1 else (3, 1)
+    if h < 1 or w < 1 or tuple(image.stride())[1:] != inner or (h > 1 and image.stride(0) < w * channels):
+        raise ValueError("deflate_strips: pixels must be packed along rows, got shape %s strides %s"
+                         % (tuple(image.shape), tuple(image.stride())))
+    f = _lib.RASTER_FORMAT[fmt]
+    bpp = _lib.RASTER_BPP[f]
+    rps = _deflate_rows(w * bpp, h, rows_per_strip)
+    device = image.device.index if image.device.index is not None else torch.cuda.current_device()
+    ctx = _jpeg_context(device)
+    torch.cuda.current_stream(image.device).synchronize()
+    stride = image.stride(0) * image.element_size() if h > 1 else w * bpp
+    data, counts = _deflate_call(
+        lambda buf, cap, size, sb: lib().amb_deflate_strips_device(ctx, C.c_void_p(image.data_ptr()), w, h, stride, f,
+                                                                   rps, buf, cap, size, sb), w, h, f, rps, ctx)
+    return data, counts, rps

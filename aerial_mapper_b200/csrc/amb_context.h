@@ -180,6 +180,9 @@ struct amb_ctx {
   amb::DeviceBuffer jpeg_spine;   // ... tile sums of its scans
   amb::DeviceBuffer jpeg_words;   // ... the entropy-coded stream before byte stuffing, and 0xFF counts per chunk
   amb::DeviceBuffer jpeg_out;     // ... the stuffed stream with its RST markers, copied to the host
+  amb::DeviceBuffer deflate_scratch;  // Deflate encoder (deflate_encode.cu): predicted bytes, tokens, per-segment,
+                                     // per-block and per-strip tables
+  amb::DeviceBuffer deflate_words;    // ... the zlib streams of all strips, copied to the host
   double dsm_density_hint = 0.0;  // points per cell of the whole cloud (0: derive from the points passed)
   bool dsm_debug = false;
   int dsm_stream_chunks = 4;  // (> 1, only with a host mirror of the output layer) gather + fill in column chunks, each chunk's

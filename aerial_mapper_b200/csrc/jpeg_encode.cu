@@ -27,8 +27,9 @@ namespace amb {
 namespace {
 
 constexpr int kMcuThreads = 128;
-constexpr int kScanThreads = 256, kScanPer = 8, kScanTile = kScanThreads * kScanPer;
 constexpr int kStuffThreads = 256, kStuffBytes = 16, kStuffChunk = kStuffThreads * kStuffBytes;
+
+#include "block_scan.inc"
 
 // ---- standard tables (ITU-T T.81 Annex K) -----------------------------------------------------------------------------
 const uint8_t kLumQuant[64] = {16, 11, 10, 16, 24,  40,  51,  61,  12, 12, 14, 19, 26,  58,  60,  55,
@@ -365,28 +366,6 @@ __device__ __forceinline__ unsigned int stream_byte(const uint32_t* words, unsig
   return (words[i >> 2] >> (24 - 8 * static_cast<int>(i & 3))) & 0xffu;
 }
 
-// Exclusive scan of one value per thread of a block; returns the thread's exclusive prefix, *total the block's sum
-template <int THREADS>
-__device__ __forceinline__ unsigned long long block_exclusive(unsigned long long v, unsigned long long* total) {
-  __shared__ unsigned long long warp_sums[THREADS / 32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  unsigned long long inc = v;
-  for (int o = 1; o < 32; o <<= 1) {
-    const unsigned long long u = __shfl_up_sync(0xffffffffu, inc, o);
-    if (lane >= o) inc += u;
-  }
-  if (lane == 31) warp_sums[warp] = inc;
-  __syncthreads();
-  unsigned long long before = 0, all = 0;
-  for (int k = 0; k < THREADS / 32; ++k) {
-    if (k < warp) before += warp_sums[k];
-    all += warp_sums[k];
-  }
-  __syncthreads();  // warp_sums is reused by the next call
-  *total = all;
-  return before + inc - v;
-}
-
 // stuff, 1: 0xFF bytes of every 4 KB chunk of the stream
 __global__ void __launch_bounds__(kStuffThreads)
     jpeg_ff_count_kernel(const uint32_t* __restrict__ words, unsigned long long n_bytes,
@@ -436,64 +415,6 @@ __global__ void __launch_bounds__(kStuffThreads)
       ++ff;
     }
   }
-}
-
-// ---- exclusive scan of n uint64 in place, a[n] = total (tile sums -> one-block spine -> tiles) ---------------------
-__global__ void __launch_bounds__(kScanThreads)
-    scan_tile_sums_kernel(const unsigned long long* __restrict__ a, unsigned long long n,
-                          unsigned long long* __restrict__ sums) {
-  const unsigned long long base = static_cast<unsigned long long>(blockIdx.x) * kScanTile + threadIdx.x * kScanPer;
-  unsigned long long v = 0;
-  for (int k = 0; k < kScanPer; ++k)
-    if (base + k < n) v += a[base + k];
-  unsigned long long total;
-  block_exclusive<kScanThreads>(v, &total);
-  if (threadIdx.x == 0) sums[blockIdx.x] = total;
-}
-
-__global__ void __launch_bounds__(1024) scan_spine_kernel(unsigned long long* __restrict__ sums, unsigned long long n,
-                                                          unsigned long long* __restrict__ total) {
-  __shared__ unsigned long long carry_s;
-  if (threadIdx.x == 0) carry_s = 0;
-  __syncthreads();
-  for (unsigned long long base = 0; base < n; base += 1024) {
-    const unsigned long long k = base + threadIdx.x;
-    const unsigned long long v = k < n ? sums[k] : 0ull;
-    unsigned long long all;
-    const unsigned long long ex = block_exclusive<1024>(v, &all) + carry_s;
-    if (k < n) sums[k] = ex;
-    __syncthreads();
-    if (threadIdx.x == 0) carry_s += all;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) *total = carry_s;
-}
-
-__global__ void __launch_bounds__(kScanThreads)
-    scan_apply_kernel(unsigned long long* __restrict__ a, unsigned long long n,
-                      const unsigned long long* __restrict__ sums) {
-  const unsigned long long base = static_cast<unsigned long long>(blockIdx.x) * kScanTile + threadIdx.x * kScanPer;
-  unsigned long long v[kScanPer], sum = 0;
-#pragma unroll
-  for (int k = 0; k < kScanPer; ++k) {
-    v[k] = base + k < n ? a[base + k] : 0ull;
-    sum += v[k];
-  }
-  unsigned long long total;
-  unsigned long long run = sums[blockIdx.x] + block_exclusive<kScanThreads>(sum, &total);
-#pragma unroll
-  for (int k = 0; k < kScanPer; ++k) {
-    if (base + k < n) a[base + k] = run;
-    run += v[k];
-  }
-}
-
-// a: n + 1 elements; spine: scratch of at least ceil(n / kScanTile) elements
-void scan_u64(unsigned long long* a, unsigned long long n, unsigned long long* spine, cudaStream_t st) {
-  const unsigned long long tiles = (n + kScanTile - 1) / kScanTile;
-  scan_tile_sums_kernel<<<static_cast<unsigned int>(tiles), kScanThreads, 0, st>>>(a, n, spine);
-  scan_spine_kernel<<<1, 1024, 0, st>>>(spine, tiles, a + n);
-  scan_apply_kernel<<<static_cast<unsigned int>(tiles), kScanThreads, 0, st>>>(a, n, spine);
 }
 
 // ---- host side -------------------------------------------------------------------------------------------------------
@@ -625,12 +546,6 @@ std::vector<unsigned char> jpeg_header(const JpegParams& p) {
 
 unsigned int grid_of(unsigned long long n, int threads) {
   return static_cast<unsigned int>((n + threads - 1) / threads);
-}
-
-int read_u64(amb_ctx* ctx, const unsigned long long* d, unsigned long long* v) {
-  AMB_CUDA(ctx, cudaMemcpyAsync(v, d, sizeof(*v), cudaMemcpyDeviceToHost, ctx->stream));
-  AMB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return AMB_OK;
 }
 
 int jpeg_encode(amb_ctx* ctx, const unsigned char* d_img, size_t row_stride, const JpegParams& p, void* host_out,

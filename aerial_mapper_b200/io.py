@@ -9,6 +9,7 @@
 and the output side ("next" row N4):
 
     write_geotiff                   :349-509   toGeoTiff / writeDataToDEMGeoTiffColor, with the map's geotransform
+    write_geotiff_strips                        the same tags around Deflate strips compressed on the device
 
 and back in: read_geotiff, the DEM GeoTIFFs GDAL writes (GridMap.from_raster resamples them into a layer).
 """
@@ -150,21 +151,14 @@ def load_camera_rig_from_file(filename_ncameras_yaml, camera_index=0):
                    tuple(_quat_from_matrix(R_C_B)), tuple(t_C_B))
 
 
-# ---- GeoTIFF (baseline TIFF 6.0 + GeoTIFF 1.0 tags), little-endian, uncompressed strips ----
+# ---- GeoTIFF (baseline TIFF 6.0 + GeoTIFF 1.0 tags), little-endian, uncompressed or Deflate strips ----
 _SHORT, _ASCII, _LONG, _DOUBLE = 3, 2, 4, 12
 _TYPE_FMT = {_SHORT: "H", _LONG: "I", _DOUBLE: "d"}
 _STRIP_BYTES = 1 << 20
 
 
-def write_geotiff(path, raster, geotransform, epsg=32632, nodata=None):
-    """io::AerialMapperIO::toGeoTiff (aerial-mapper-io.cc:349-509) with the map's own geotransform: a north-up raster
-    whose GDAL-order `geotransform` is (west, res_x, 0, north, 0, -res_y) (GridMap.geotransform()), in the projected CRS
-    `epsg` (default: the reference's hard-coded UTM zone 32N, :391-393).
-
-    raster: uint8 or float32 [H, W] (one band; float32 is written with SampleFormat 3), or uint8 [H, W, 3] in B, G, R
-    order (GridMap.to_raster(.., "bgr8")), stored as RGB one strip at a time.  nodata: GDAL_NODATA, e.g. "nan" for a DEM
-    with NaN as no-data.  Uncompressed, no BigTIFF: a file over 4 GiB raises ValueError."""
-    a = np.asarray(raster)
+def _check_raster(a):
+    """(bands, bits) of a raster write_geotiff accepts, else ValueError."""
     if a.ndim == 2 and a.dtype in (np.uint8, np.float32):
         bands = 1
     elif a.ndim == 3 and a.shape[2] == 3 and a.dtype == np.uint8:
@@ -172,29 +166,34 @@ def write_geotiff(path, raster, geotransform, epsg=32632, nodata=None):
     else:
         raise ValueError("raster must be uint8 or float32 [H, W], or uint8 [H, W, 3] (B, G, R); got %s %r"
                          % (a.dtype, a.shape))
-    height, width = a.shape[:2]
-    if height < 1 or width < 1:
+    if a.shape[0] < 1 or a.shape[1] < 1:
         raise ValueError("empty raster")
+    return bands, (32 if a.dtype == np.float32 else 8)
+
+
+def _tiff_layout(width, height, bands, bits, rows_per_strip, strip_counts, geotransform, epsg, nodata,
+                 predictor=None):
+    """The file's bytes up to its first strip (header, the one IFD, its out-of-line values, zero padding to a 16-byte
+    boundary), for strips of `strip_counts` bytes stored back to back after it.  predictor: None for uncompressed
+    strips, else Compression 8 (Deflate) with that Predictor.  A file over 4 GiB raises ValueError (no BigTIFF)."""
     gt = [float(v) for v in geotransform]
     if len(gt) != 6 or gt[2] != 0.0 or gt[4] != 0.0 or not gt[1] > 0.0 or not gt[5] < 0.0:
         raise ValueError("a north-up geotransform (x0, res, 0, y0, 0, -res) is required, got %r" % (gt,))
-    bits = 32 if a.dtype == np.float32 else 8
-    row_bytes = width * bands * bits // 8
-    rows_per_strip = max(1, min(height, _STRIP_BYTES // row_bytes))
-    n_strips = (height + rows_per_strip - 1) // rows_per_strip
-    strip_counts = [min(rows_per_strip, height - s * rows_per_strip) * row_bytes for s in range(n_strips)]
-
+    n_strips = len(strip_counts)
     geokeys = [1, 1, 0, 3,                 # GeoKeyDirectory header: version 1.1.0, 3 keys
                1024, 0, 1, 1,              # GTModelTypeGeoKey = ModelTypeProjected
                1025, 0, 1, 1,              # GTRasterTypeGeoKey = RasterPixelIsArea
                3072, 0, 1, int(epsg)]      # ProjectedCSTypeGeoKey
-    tags = [(256, _LONG, [width]), (257, _LONG, [height]), (258, _SHORT, [bits] * bands), (259, _SHORT, [1]),
+    tags = [(256, _LONG, [width]), (257, _LONG, [height]), (258, _SHORT, [bits] * bands),
+            (259, _SHORT, [1 if predictor is None else 8]),
             (262, _SHORT, [2 if bands == 3 else 1]), (273, _LONG, [0] * n_strips), (277, _SHORT, [bands]),
-            (278, _LONG, [rows_per_strip]), (279, _LONG, strip_counts), (284, _SHORT, [1]),
-            (339, _SHORT, [3 if bits == 32 else 1] * bands),
-            (33550, _DOUBLE, [gt[1], -gt[5], 0.0]),                  # ModelPixelScale
-            (33922, _DOUBLE, [0.0, 0.0, 0.0, gt[0], gt[3], 0.0]),    # ModelTiepoint: pixel corner (0, 0) -> (west, north)
-            (34735, _SHORT, geokeys)]
+            (278, _LONG, [rows_per_strip]), (279, _LONG, list(strip_counts)), (284, _SHORT, [1])]
+    if predictor is not None:
+        tags.append((317, _SHORT, [predictor]))
+    tags += [(339, _SHORT, [3 if bits == 32 else 1] * bands),
+             (33550, _DOUBLE, [gt[1], -gt[5], 0.0]),                  # ModelPixelScale
+             (33922, _DOUBLE, [0.0, 0.0, 0.0, gt[0], gt[3], 0.0]),    # ModelTiepoint: pixel corner (0, 0) -> (west, north)
+             (34735, _SHORT, geokeys)]
     if nodata is not None:
         tags.append((42113, _ASCII, ("%s" % nodata).encode("ascii") + b"\0"))   # GDAL_NODATA
 
@@ -209,8 +208,8 @@ def write_geotiff(path, raster, geotransform, epsg=32632, nodata=None):
     total = data_at + sum(strip_counts)
     if total > 0xFFFFFFFF:
         raise ValueError("%d bytes: larger than a classic TIFF can address (4 GiB); BigTIFF is not supported" % total)
-    offsets = [data_at + sum(strip_counts[:s]) for s in range(n_strips)]
-    tags[5] = (273, _LONG, offsets)
+    offsets = np.concatenate([[0], np.cumsum(np.asarray(strip_counts, np.int64))[:-1]]) + data_at
+    tags[5] = (273, _LONG, [int(v) for v in offsets])
 
     ifd = struct.pack("<H", len(tags))
     blobs = b""
@@ -223,14 +222,53 @@ def write_geotiff(path, raster, geotransform, epsg=32632, nodata=None):
             ifd += struct.pack("<HHII", tag, typ, count, extra_at + len(blobs))
             blobs += p + (b"\0" if len(p) & 1 else b"")
     ifd += struct.pack("<I", 0)
+    head = b"II*\0" + struct.pack("<I", ifd_at) + ifd + blobs
+    return head + b"\0" * (data_at - len(head))
+
+
+def write_geotiff(path, raster, geotransform, epsg=32632, nodata=None):
+    """io::AerialMapperIO::toGeoTiff (aerial-mapper-io.cc:349-509) with the map's own geotransform: a north-up raster
+    whose GDAL-order `geotransform` is (west, res_x, 0, north, 0, -res_y) (GridMap.geotransform()), in the projected CRS
+    `epsg` (default: the reference's hard-coded UTM zone 32N, :391-393).
+
+    raster: uint8 or float32 [H, W] (one band; float32 is written with SampleFormat 3), or uint8 [H, W, 3] in B, G, R
+    order (GridMap.to_raster(.., "bgr8")), stored as RGB one strip at a time.  nodata: GDAL_NODATA, e.g. "nan" for a DEM
+    with NaN as no-data.  Uncompressed, no BigTIFF: a file over 4 GiB raises ValueError.  GridMap.to_geotiff writes
+    Deflate-compressed files."""
+    a = np.asarray(raster)
+    bands, bits = _check_raster(a)
+    height, width = a.shape[:2]
+    row_bytes = width * bands * bits // 8
+    rows_per_strip = max(1, min(height, _STRIP_BYTES // row_bytes))
+    n_strips = (height + rows_per_strip - 1) // rows_per_strip
+    strip_counts = [min(rows_per_strip, height - s * rows_per_strip) * row_bytes for s in range(n_strips)]
+    head = _tiff_layout(width, height, bands, bits, rows_per_strip, strip_counts, geotransform, epsg, nodata)
     with open(path, "wb") as f:
-        f.write(b"II*\0" + struct.pack("<I", ifd_at) + ifd + blobs)
-        f.write(b"\0" * (data_at - f.tell()))
+        f.write(head)
         for s in range(n_strips):
             part = a[s * rows_per_strip:(s + 1) * rows_per_strip]
             if bands == 3:
                 part = part[:, :, ::-1]               # B, G, R -> R, G, B, this strip only
             f.write(np.ascontiguousarray(part, dtype=a.dtype.newbyteorder("<")).tobytes())
+
+
+def write_geotiff_strips(path, data, strip_bytes, width, height, fmt, rows_per_strip, geotransform, epsg=32632,
+                         nodata=None):
+    """Writes Deflate-compressed strips (GridMap.to_geotiff, deflate_strips; convention in include/aerial_mapper_b200.h,
+    amb_deflate_strips_device) as a GeoTIFF with the tags write_geotiff writes, plus Compression 8 and Predictor 3 for
+    fmt "f32", 2 for "gray8", "bgr8" and "mask8".  data: the strips back to back; strip_bytes: each strip's length."""
+    bands, bits, predictor = {"f32": (1, 32, 3), "gray8": (1, 8, 2), "bgr8": (3, 8, 2), "mask8": (1, 8, 2)}[fmt]
+    data = memoryview(data).cast("B")
+    counts = [int(v) for v in strip_bytes]
+    rps = int(rows_per_strip)
+    if width < 1 or height < 1 or rps < 1 or len(counts) != (height + rps - 1) // rps or sum(counts) != len(data):
+        raise ValueError("write_geotiff_strips: %d strips of %d bytes in all do not fit a %d x %d raster in strips of %d "
+                         "rows" % (len(counts), sum(counts), width, height, rps))
+    head = _tiff_layout(int(width), int(height), bands, bits, min(rps, int(height)), counts, geotransform, epsg, nodata,
+                        predictor)
+    with open(path, "wb") as f:
+        f.write(head)
+        f.write(data)
 
 
 # ---- GeoTIFF reader: the subset GDAL writes for DEMs ----

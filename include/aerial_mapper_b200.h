@@ -523,6 +523,40 @@ int amb_jpeg_encode_device(amb_ctx* ctx, const void* d_image, int32_t width, int
 int amb_export_jpeg(amb_ctx* ctx, int layer, int format, int quality, int sampling, int32_t restart_interval,
                     void* host_out, size_t capacity, size_t* size);
 
+/* ---- Deflate-compressed GeoTIFF strips ----
+ * Convention.  The strips of a classic TIFF with Compression = 8 (Adobe Deflate), PlanarConfiguration 1 and
+ * RowsPerStrip = rows_per_strip (a value over height means one strip), for a raster in one of the export's formats
+ * (amb_raster_format; BGR8 arrives as B, G, R and is stored as R, G, B):
+ *   Predictor 3 for AMB_RASTER_F32 (libtiff's floating-point predictor): each row's samples become big-endian byte
+ *     planes, most significant plane first, then every byte but the row's first is replaced by its difference (mod 256)
+ *     with the byte before it;
+ *   Predictor 2 for AMB_RASTER_GRAY8, AMB_RASTER_BGR8, AMB_RASTER_MASK8: within each row, byte k minus byte k - spp,
+ *     mod 256 (spp = 3 for BGR8, else 1).
+ * Every strip (its rows' predicted bytes, n of them) is one zlib stream (RFC 1950 header 78 01, RFC 1951 blocks of at
+ * most 65535 bytes each, the Adler-32 of the n bytes); matches never reach outside the strip, Huffman codes are at most
+ * 15 bits and code-length codes at most 7.  A block whose coded size would exceed its stored size is stored, so a
+ * strip is never longer than n + 5 ceil(n / 65535) + 6 bytes.  The bytes are a function of the raster, the format and
+ * rows_per_strip only (not of the device, the launch schedule or earlier calls); they decode exactly, with zlib or any
+ * TIFF reader, but are not promised to equal what zlib would write.
+ * Errors: a NULL pointer, a bad format, width, height or rows_per_strip <= 0, a row_stride below the row's bytes, or an
+ * F32 image or stride that is not a multiple of 4 bytes returns AMB_ERR_INVALID_ARGUMENT; a strip whose bound exceeds
+ * 4 GiB AMB_ERR_UNSUPPORTED.  Neither writes anything. */
+/* Host arithmetic, no GPU: the sum of the strips' bounds above; 0 if the arguments are invalid or unsupported. */
+size_t amb_deflate_max_size(int32_t width, int32_t height, int format, int32_t rows_per_strip);
+/* Compresses a device raster valid on the context's device (8-bit formats at any byte alignment), ordered after
+ * earlier work on the context's stream.  Synchronous: on return the strips are in host_out back to back (*size bytes,
+ * pinned or pageable) and strip_bytes[ceil(height / rows_per_strip)] holds each strip's length.  If capacity < *size it
+ * returns AMB_ERR_SIZE_MISMATCH with the size needed in *size and writes nothing else.  Device scratch, kept by the
+ * context: about 4.4x the raster's bytes at 8 KiB strips, plus ~1.3 KB per 13107 bytes of a strip and ~1.8 KB per
+ * strip, so very short strips cost more than the raster. */
+int amb_deflate_strips_device(amb_ctx* ctx, const void* d_image, int32_t width, int32_t height, size_t row_stride,
+                              int format, int32_t rows_per_strip, void* host_out, size_t capacity, size_t* size,
+                              uint32_t* strip_bytes);
+/* amb_export_raster_device of `layer` in `format` into the context's scratch, then amb_deflate_strips_device of it: the
+ * context's band (image rows [col_begin, col_end)) as an image of its own. */
+int amb_export_deflate_strips(amb_ctx* ctx, int layer, int format, int32_t rows_per_strip, void* host_out,
+                              size_t capacity, size_t* size, uint32_t* strip_bytes);
+
 /* ---- measurement ---- */
 int amb_get_timings(amb_ctx* ctx, amb_timings* out);
 
