@@ -162,6 +162,11 @@ SYMBOLS = {
                                             C.c_size_t, C.POINTER(C.c_size_t), _P]),
     "amb_export_deflate_strips": (C.c_int, [_P, C.c_int, C.c_int, C.c_int32, _P, C.c_size_t, C.POINTER(C.c_size_t),
                                             _P]),
+    "amb_cog_layout": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, _P, _P, _P]),
+    "amb_cog_max_size": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int, C.c_int32]),
+    "amb_cog_tiles_device": (C.c_int, [_P, _P, C.c_int32, C.c_int32, C.c_size_t, C.c_int, C.c_int32, _P, C.c_size_t,
+                                       C.POINTER(C.c_size_t), _P]),
+    "amb_export_cog_tiles": (C.c_int, [_P, C.c_int, C.c_int, C.c_int32, _P, C.c_size_t, C.POINTER(C.c_size_t), _P]),
     "amb_get_timings": (C.c_int, [_P, C.POINTER(Timings)]),
     "amb_host_alloc": (C.c_int, [C.POINTER(_P), C.c_size_t]),
     "amb_host_free": (C.c_int, [_P]),

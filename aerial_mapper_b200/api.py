@@ -286,6 +286,34 @@ class GridMap(object):
         from . import io
         io.write_geotiff_strips(path, data, counts, width, height, fmt, rps, gt, epsg, nodata)
 
+    def to_cog(self, path, name, fmt=None, epsg=32632, nodata=None, tile_size=512):
+        """Writes the context's band of layer `name` to `path` as a Cloud-Optimized GeoTIFF: T x T Deflate tiles with
+        internal overviews halved until one fits a tile, pyramid, tiles and compression on the device (convention:
+        include/aerial_mapper_b200.h, amb_cog_tiles_device; layout: io.write_cog).  Level 0 reads back as to_raster(name,
+        fmt) bit for bit.  fmt and the geotransform as to_geotiff.  nodata must agree with the overviews: "nan" (or NaN)
+        for "f32", 0 for "mask8", none for "gray8" and "bgr8".  tile_size: a multiple of 16 in [16, 4096]."""
+        if not self._resident:
+            raise AmbError(_lib.AMB_ERR_INVALID_ARGUMENT, "to_cog exports device-resident layers: call to_device() first")
+        if fmt is None:
+            fmt = {"elevation": "f32", "ortho": "gray8", "colored_ortho": "bgr8"}.get(name)
+            if fmt is None:
+                raise ValueError("to_cog(%r): give fmt='f32', 'gray8', 'bgr8' or 'mask8' for this layer" % (name,))
+        if fmt not in _lib.RASTER_FORMAT:
+            raise ValueError("to_cog: fmt must be 'f32', 'gray8', 'bgr8' or 'mask8', got %r" % (fmt,))
+        from . import io
+        io.cog_nodata(fmt, nodata)
+        tile = _cog_tile(tile_size)
+        f = _lib.RASTER_FORMAT[fmt]
+        c0, c1 = self._col_range
+        width, height = self.geometry.rows, c1 - c0
+        ctx = self._ctx
+        data, counts = _cog_call(
+            lambda buf, cap, size, tb: lib().amb_export_cog_tiles(ctx, LAYER_ID[name], f, tile, buf, cap, size, tb),
+            width, height, f, tile, ctx)
+        gt = list(self.geotransform())
+        gt[3] += c0 * gt[5]        # the band's north edge
+        io.write_cog(path, data, counts, width, height, fmt, tile, gt, epsg, nodata)
+
     def timings(self):
         t = _lib.Timings()
         check(lib().amb_get_timings(self.context(), C.byref(t)), self._ctx)
@@ -797,35 +825,76 @@ def _deflate_call(call, width, height, fmt, rps, ctx):
 _DEFLATE_DTYPES = {"f32": "float32", "gray8": "uint8", "mask8": "uint8", "bgr8": "uint8"}
 
 
+def _device_raster(image, fmt, what):
+    """Checks a torch CUDA raster of format `fmt` for deflate_strips / cog_tiles (ValueError otherwise); returns (h, w,
+    format id, row stride in bytes, the device's context) once the work queued on the current torch stream is done."""
+    import torch
+    if fmt not in _DEFLATE_DTYPES:
+        raise ValueError("%s: fmt must be 'f32', 'gray8', 'bgr8' or 'mask8', got %r" % (what, fmt))
+    if not isinstance(image, torch.Tensor) or not image.is_cuda or \
+            image.dtype != getattr(torch, _DEFLATE_DTYPES[fmt]):
+        raise ValueError("%s: expected a torch CUDA %s tensor for %r" % (what, _DEFLATE_DTYPES[fmt], fmt))
+    channels = 3 if fmt == "bgr8" else 1
+    if image.dim() != (3 if channels == 3 else 2) or (channels == 3 and image.shape[2] != 3):
+        raise ValueError("%s: expected %s for %r, got %s"
+                         % (what, "H x W x 3" if channels == 3 else "H x W", fmt, tuple(image.shape)))
+    h, w = int(image.shape[0]), int(image.shape[1])
+    inner = (1,) if channels == 1 else (3, 1)
+    if h < 1 or w < 1 or tuple(image.stride())[1:] != inner or (h > 1 and image.stride(0) < w * channels):
+        raise ValueError("%s: pixels must be packed along rows, got shape %s strides %s"
+                         % (what, tuple(image.shape), tuple(image.stride())))
+    f = _lib.RASTER_FORMAT[fmt]
+    device = image.device.index if image.device.index is not None else torch.cuda.current_device()
+    ctx = _jpeg_context(device)
+    torch.cuda.current_stream(image.device).synchronize()
+    stride = image.stride(0) * image.element_size() if h > 1 else w * _lib.RASTER_BPP[f]
+    return h, w, f, stride, ctx
+
+
 def deflate_strips(image, fmt, rows_per_strip=None):
     """The Deflate-compressed GeoTIFF strips of a torch CUDA raster, compressed on its device (convention:
     include/aerial_mapper_b200.h, amb_deflate_strips_device): returns (strips as bytes, uint32 length of each strip,
     rows_per_strip), ready for io.write_geotiff_strips.  image: float32 H x W for fmt "f32", uint8 H x W for "gray8" and
     "mask8", uint8 H x W x 3 (B, G, R) for "bgr8".  Rows may be padded (a row-sliced view), pixels must be packed.  Waits
     for the work queued on the current torch stream before reading the image."""
-    import torch
-    if fmt not in _DEFLATE_DTYPES:
-        raise ValueError("deflate_strips: fmt must be 'f32', 'gray8', 'bgr8' or 'mask8', got %r" % (fmt,))
-    if not isinstance(image, torch.Tensor) or not image.is_cuda or \
-            image.dtype != getattr(torch, _DEFLATE_DTYPES[fmt]):
-        raise ValueError("deflate_strips: expected a torch CUDA %s tensor for %r" % (_DEFLATE_DTYPES[fmt], fmt))
-    channels = 3 if fmt == "bgr8" else 1
-    if image.dim() != (3 if channels == 3 else 2) or (channels == 3 and image.shape[2] != 3):
-        raise ValueError("deflate_strips: expected %s for %r, got %s"
-                         % ("H x W x 3" if channels == 3 else "H x W", fmt, tuple(image.shape)))
-    h, w = int(image.shape[0]), int(image.shape[1])
-    inner = (1,) if channels == 1 else (3, 1)
-    if h < 1 or w < 1 or tuple(image.stride())[1:] != inner or (h > 1 and image.stride(0) < w * channels):
-        raise ValueError("deflate_strips: pixels must be packed along rows, got shape %s strides %s"
-                         % (tuple(image.shape), tuple(image.stride())))
-    f = _lib.RASTER_FORMAT[fmt]
-    bpp = _lib.RASTER_BPP[f]
-    rps = _deflate_rows(w * bpp, h, rows_per_strip)
-    device = image.device.index if image.device.index is not None else torch.cuda.current_device()
-    ctx = _jpeg_context(device)
-    torch.cuda.current_stream(image.device).synchronize()
-    stride = image.stride(0) * image.element_size() if h > 1 else w * bpp
+    h, w, f, stride, ctx = _device_raster(image, fmt, "deflate_strips")
+    rps = _deflate_rows(w * _lib.RASTER_BPP[f], h, rows_per_strip)
     data, counts = _deflate_call(
         lambda buf, cap, size, sb: lib().amb_deflate_strips_device(ctx, C.c_void_p(image.data_ptr()), w, h, stride, f,
                                                                    rps, buf, cap, size, sb), w, h, f, rps, ctx)
     return data, counts, rps
+
+
+# ---- Cloud-Optimized GeoTIFF tiles (amb_cog_tiles_device, amb_export_cog_tiles) ------------------------------------------
+def _cog_tile(tile_size):
+    if isinstance(tile_size, bool) or not isinstance(tile_size, (int, np.integer)) or not 16 <= tile_size <= 4096 or \
+            tile_size % 16:
+        raise ValueError("tile_size must be a multiple of 16 in [16, 4096], got %r" % (tile_size,))
+    return int(tile_size)
+
+
+def _cog_call(call, width, height, fmt, tile, ctx):
+    """Runs `call(buffer, capacity, size, tile_bytes)` with a buffer of amb_cog_max_size bytes; returns the tiles in file
+    order (bytes) and their lengths (uint32 array)."""
+    cap = lib().amb_cog_max_size(width, height, fmt, tile)
+    if cap == 0:
+        raise AmbError(_lib.AMB_ERR_UNSUPPORTED, "a %d x %d raster in tiles of %d" % (width, height, tile))
+    from . import io
+    n_tiles = sum(-(-w // tile) * -(-h // tile) for w, h in io.cog_layout(width, height, tile))
+    buf = np.empty(cap, np.uint8)
+    counts = np.zeros(n_tiles, np.uint32)
+    size = C.c_size_t(0)
+    check(call(buf.ctypes.data_as(C.c_void_p), cap, C.byref(size), counts.ctypes.data_as(C.c_void_p)), ctx)
+    return buf[:size.value].tobytes(), counts
+
+
+def cog_tiles(image, fmt, tile_size=512):
+    """The tiles of a Cloud-Optimized GeoTIFF of a torch CUDA raster: overview pyramid, tiling and Deflate on its device
+    (convention: include/aerial_mapper_b200.h, amb_cog_tiles_device).  Returns (tiles as bytes in file order, uint32
+    length of each tile), ready for io.write_cog.  image and fmt as for deflate_strips; tile_size a multiple of 16 in
+    [16, 4096].  Waits for the work queued on the current torch stream before reading the image."""
+    tile = _cog_tile(tile_size)
+    h, w, f, stride, ctx = _device_raster(image, fmt, "cog_tiles")
+    return _cog_call(
+        lambda buf, cap, size, tb: lib().amb_cog_tiles_device(ctx, C.c_void_p(image.data_ptr()), w, h, stride, f, tile,
+                                                              buf, cap, size, tb), w, h, f, tile, ctx)

@@ -183,6 +183,9 @@ struct amb_ctx {
   amb::DeviceBuffer deflate_scratch;  // Deflate encoder (deflate_encode.cu): predicted bytes, tokens, per-segment,
                                      // per-block and per-strip tables
   amb::DeviceBuffer deflate_words;    // ... the zlib streams of all strips, copied to the host
+  amb::DeviceBuffer cog_levels;       // Cloud-Optimized GeoTIFF (raster_pyramid.cu): the overview levels 1.., rows padded
+                                      // to 16 bytes, one after another
+  amb::DeviceBuffer cog_tiles;        // ... every level's tiles stacked into one raster T wide, compressed as T-row strips
   double dsm_density_hint = 0.0;  // points per cell of the whole cloud (0: derive from the points passed)
   bool dsm_debug = false;
   int dsm_stream_chunks = 4;  // (> 1, only with a host mirror of the output layer) gather + fill in column chunks, each chunk's

@@ -21,7 +21,7 @@
 #include <algorithm>
 #include <cstring>
 
-#include "amb_context.h"
+#include "deflate_encode.h"
 
 namespace amb {
 namespace {
@@ -43,20 +43,6 @@ constexpr unsigned kAdlerMod = 65521u;
 // token words (uint16 per predicted byte): a token start holds 0x8000 | literal or 0x8100 + (length - 3), the byte
 // after a match start its distance - 1 (< 0x8000); every other byte kNone
 constexpr uint16_t kNone = 0xFFFFu, kLit = 0x8000u, kMatch = 0x8100u;
-
-struct DeflateShape {
-  const unsigned char* img;
-  unsigned long long stride;     // bytes between raster rows
-  int32_t w, h;
-  int32_t spp, bps;              // samples per pixel, bytes per sample
-  unsigned long long row_bytes;  // predicted bytes per row = w * spp * bps
-  int32_t rps;                   // rows per strip
-  int32_t n_strips;
-  int32_t segs;                  // segments per full strip
-  int32_t blocks;                // blocks per full strip
-  int32_t win_bytes, prev_bytes; // the match kernel's shared memory: the largest window and its segment's chain links,
-                                 // each rounded up to 16 bytes (strips shorter than a window take less)
-};
 
 __device__ __forceinline__ unsigned long long min_u64(unsigned long long a, unsigned long long b) { return a < b ? a : b; }
 
@@ -766,15 +752,12 @@ __global__ void __launch_bounds__(128)
 }
 
 // ---- host side ------------------------------------------------------------------------------------------------------------
-struct DeflateParams {
-  DeflateShape s;
-  unsigned long long n_bytes;  // predicted bytes of the whole raster
-  unsigned long long bound;    // the largest file
-};
-
 unsigned long long strip_bound(unsigned long long n) { return n + 5 * ((n + kBlock - 1) / kBlock) + 6; }
 
-// AMB_OK, AMB_ERR_INVALID_ARGUMENT or AMB_ERR_UNSUPPORTED (a strip over 4 GiB, which TIFF cannot count)
+size_t align256(size_t v) { return (v + 255) & ~size_t(255); }
+
+}  // namespace
+
 int deflate_params(int32_t w, int32_t h, int format, int32_t rps, DeflateParams* p) {
   if (w <= 0 || h <= 0 || rps <= 0) return AMB_ERR_INVALID_ARGUMENT;
   DeflateShape& s = p->s;
@@ -806,8 +789,6 @@ int deflate_params(int32_t w, int32_t h, int format, int32_t rps, DeflateParams*
   p->bound = strip_bound(full) * (s.n_strips - 1) + strip_bound(last);
   return AMB_OK;
 }
-
-size_t align256(size_t v) { return (v + 255) & ~size_t(255); }
 
 int deflate_encode(amb_ctx* ctx, const unsigned char* d_img, size_t row_stride, DeflateParams p, void* host_out,
                    size_t capacity, size_t* size, uint32_t* strip_bytes) {
@@ -878,7 +859,6 @@ int deflate_encode(amb_ctx* ctx, const unsigned char* d_img, size_t row_stride, 
   return staged_d2h(ctx, strip_bytes, lens32, static_cast<size_t>(S) * 4, st);
 }
 
-}  // namespace
 }  // namespace amb
 
 using namespace amb;

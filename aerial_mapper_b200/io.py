@@ -13,6 +13,7 @@ and the output side ("next" row N4):
 
 and back in: read_geotiff, the DEM GeoTIFFs GDAL writes (GridMap.from_raster resamples them into a layer).
 """
+import ctypes as C
 import math
 import os
 import struct
@@ -171,58 +172,89 @@ def _check_raster(a):
     return bands, (32 if a.dtype == np.float32 else 8)
 
 
-def _tiff_layout(width, height, bands, bits, rows_per_strip, strip_counts, geotransform, epsg, nodata,
-                 predictor=None):
-    """The file's bytes up to its first strip (header, the one IFD, its out-of-line values, zero padding to a 16-byte
-    boundary), for strips of `strip_counts` bytes stored back to back after it.  predictor: None for uncompressed
-    strips, else Compression 8 (Deflate) with that Predictor.  A file over 4 GiB raises ValueError (no BigTIFF)."""
+def _north_up(geotransform):
     gt = [float(v) for v in geotransform]
     if len(gt) != 6 or gt[2] != 0.0 or gt[4] != 0.0 or not gt[1] > 0.0 or not gt[5] < 0.0:
         raise ValueError("a north-up geotransform (x0, res, 0, y0, 0, -res) is required, got %r" % (gt,))
-    n_strips = len(strip_counts)
-    geokeys = [1, 1, 0, 3,                 # GeoKeyDirectory header: version 1.1.0, 3 keys
-               1024, 0, 1, 1,              # GTModelTypeGeoKey = ModelTypeProjected
-               1025, 0, 1, 1,              # GTRasterTypeGeoKey = RasterPixelIsArea
-               3072, 0, 1, int(epsg)]      # ProjectedCSTypeGeoKey
+    return gt
+
+
+def _image_tags(width, height, bands, bits, predictor, layout, geo=None, subfile=None):
+    """The tags of one image's IFD in ascending order: `layout` holds its strip or tile tags; predictor None for
+    uncompressed data, else Compression 8 (Deflate) with that Predictor; geo (geotransform, epsg, nodata) adds the
+    georeferencing; subfile, if given, NewSubfileType (0 full resolution, 1 reduced)."""
     tags = [(256, _LONG, [width]), (257, _LONG, [height]), (258, _SHORT, [bits] * bands),
-            (259, _SHORT, [1 if predictor is None else 8]),
-            (262, _SHORT, [2 if bands == 3 else 1]), (273, _LONG, [0] * n_strips), (277, _SHORT, [bands]),
-            (278, _LONG, [rows_per_strip]), (279, _LONG, list(strip_counts)), (284, _SHORT, [1])]
+            (259, _SHORT, [1 if predictor is None else 8]), (262, _SHORT, [2 if bands == 3 else 1]),
+            (277, _SHORT, [bands]), (284, _SHORT, [1]), (339, _SHORT, [3 if bits == 32 else 1] * bands)]
+    tags += list(layout)
+    if subfile is not None:
+        tags.append((254, _LONG, [subfile]))
     if predictor is not None:
         tags.append((317, _SHORT, [predictor]))
-    tags += [(339, _SHORT, [3 if bits == 32 else 1] * bands),
-             (33550, _DOUBLE, [gt[1], -gt[5], 0.0]),                  # ModelPixelScale
-             (33922, _DOUBLE, [0.0, 0.0, 0.0, gt[0], gt[3], 0.0]),    # ModelTiepoint: pixel corner (0, 0) -> (west, north)
-             (34735, _SHORT, geokeys)]
-    if nodata is not None:
-        tags.append((42113, _ASCII, ("%s" % nodata).encode("ascii") + b"\0"))   # GDAL_NODATA
+    if geo is not None:
+        gt, epsg, nodata = geo
+        geokeys = [1, 1, 0, 3,                 # GeoKeyDirectory header: version 1.1.0, 3 keys
+                   1024, 0, 1, 1,              # GTModelTypeGeoKey = ModelTypeProjected
+                   1025, 0, 1, 1,              # GTRasterTypeGeoKey = RasterPixelIsArea
+                   3072, 0, 1, int(epsg)]      # ProjectedCSTypeGeoKey
+        tags += [(33550, _DOUBLE, [gt[1], -gt[5], 0.0]),                  # ModelPixelScale
+                 (33922, _DOUBLE, [0.0, 0.0, 0.0, gt[0], gt[3], 0.0]),    # ModelTiepoint: pixel corner (0, 0) -> (west, north)
+                 (34735, _SHORT, geokeys)]
+        if nodata is not None:
+            tags.append((42113, _ASCII, ("%s" % nodata).encode("ascii") + b"\0"))   # GDAL_NODATA
+    return sorted(tags, key=lambda t: t[0])
 
-    def payload(typ, vals):
-        return bytes(vals) if typ == _ASCII else struct.pack("<%d%s" % (len(vals), _TYPE_FMT[typ]), *vals)
 
-    ifd_at = 8
-    extra_at = ifd_at + 2 + 12 * len(tags) + 4
-    # sizes of the out-of-line values, then the strip offsets once the image data's position is known
-    extra = sum((len(payload(t, v)) + 1) & ~1 for _, t, v in tags if len(payload(t, v)) > 4)
-    data_at = (extra_at + extra + 15) & ~15
-    total = data_at + sum(strip_counts)
-    if total > 0xFFFFFFFF:
-        raise ValueError("%d bytes: larger than a classic TIFF can address (4 GiB); BigTIFF is not supported" % total)
-    offsets = np.concatenate([[0], np.cumsum(np.asarray(strip_counts, np.int64))[:-1]]) + data_at
-    tags[5] = (273, _LONG, [int(v) for v in offsets])
+def _payload(typ, vals):
+    return bytes(vals) if typ == _ASCII else struct.pack("<%d%s" % (len(vals), _TYPE_FMT[typ]), *vals)
 
+
+def _ifd_size(tags):
+    """Bytes of the IFD of `tags` and its out-of-line values (each padded to an even length)."""
+    return 2 + 12 * len(tags) + 4 + sum((len(_payload(t, v)) + 1) & ~1 for _, t, v in tags if len(_payload(t, v)) > 4)
+
+
+def _set_tag(tags, tag, typ, vals):
+    return [(k, typ, list(vals)) if k == tag else (k, t, v) for k, t, v in tags]
+
+
+def _ifd(tags, at, next_ifd=0):
+    """The IFD of `tags` at file offset `at`, pointing to the next IFD at `next_ifd` (0: the last), followed by its
+    out-of-line values: _ifd_size(tags) bytes."""
+    extra_at = at + 2 + 12 * len(tags) + 4
     ifd = struct.pack("<H", len(tags))
     blobs = b""
     for tag, typ, vals in tags:
-        p = payload(typ, vals)
+        p = _payload(typ, vals)
         count = len(vals)
         if len(p) <= 4:
             ifd += struct.pack("<HHI", tag, typ, count) + p.ljust(4, b"\0")
         else:
             ifd += struct.pack("<HHII", tag, typ, count, extra_at + len(blobs))
             blobs += p + (b"\0" if len(p) & 1 else b"")
-    ifd += struct.pack("<I", 0)
-    head = b"II*\0" + struct.pack("<I", ifd_at) + ifd + blobs
+    return ifd + struct.pack("<I", next_ifd) + blobs
+
+
+def _check_size(total):
+    if total > 0xFFFFFFFF:
+        raise ValueError("%d bytes: larger than a classic TIFF can address (4 GiB); BigTIFF is not supported" % total)
+
+
+def _tiff_layout(width, height, bands, bits, rows_per_strip, strip_counts, geotransform, epsg, nodata,
+                 predictor=None):
+    """The file's bytes up to its first strip (header, the one IFD, its out-of-line values, zero padding to a 16-byte
+    boundary), for strips of `strip_counts` bytes stored back to back after it.  predictor: None for uncompressed
+    strips, else Compression 8 (Deflate) with that Predictor.  A file over 4 GiB raises ValueError (no BigTIFF)."""
+    gt = _north_up(geotransform)
+    n_strips = len(strip_counts)
+    layout = [(273, _LONG, [0] * n_strips), (278, _LONG, [rows_per_strip]), (279, _LONG, list(strip_counts))]
+    tags = _image_tags(width, height, bands, bits, predictor, layout, (gt, epsg, nodata))
+    ifd_at = 8
+    data_at = (ifd_at + _ifd_size(tags) + 15) & ~15
+    _check_size(data_at + sum(strip_counts))
+    offsets = np.concatenate([[0], np.cumsum(np.asarray(strip_counts, np.int64))[:-1]]) + data_at
+    tags = _set_tag(tags, 273, _LONG, [int(v) for v in offsets])
+    head = b"II*\0" + struct.pack("<I", ifd_at) + _ifd(tags, ifd_at)
     return head + b"\0" * (data_at - len(head))
 
 
@@ -257,7 +289,7 @@ def write_geotiff_strips(path, data, strip_bytes, width, height, fmt, rows_per_s
     """Writes Deflate-compressed strips (GridMap.to_geotiff, deflate_strips; convention in include/aerial_mapper_b200.h,
     amb_deflate_strips_device) as a GeoTIFF with the tags write_geotiff writes, plus Compression 8 and Predictor 3 for
     fmt "f32", 2 for "gray8", "bgr8" and "mask8".  data: the strips back to back; strip_bytes: each strip's length."""
-    bands, bits, predictor = {"f32": (1, 32, 3), "gray8": (1, 8, 2), "bgr8": (3, 8, 2), "mask8": (1, 8, 2)}[fmt]
+    bands, bits, predictor = _DEFLATE_FORMATS[fmt]
     data = memoryview(data).cast("B")
     counts = [int(v) for v in strip_bytes]
     rps = int(rows_per_strip)
@@ -268,6 +300,78 @@ def write_geotiff_strips(path, data, strip_bytes, width, height, fmt, rows_per_s
                         predictor)
     with open(path, "wb") as f:
         f.write(head)
+        f.write(data)
+
+
+_DEFLATE_FORMATS = {"f32": (1, 32, 3), "gray8": (1, 8, 2), "bgr8": (3, 8, 2), "mask8": (1, 8, 2)}  # bands, bits, predictor
+
+
+def cog_layout(width, height, tile):
+    """[(w_k, h_k)] of the levels of a Cloud-Optimized GeoTIFF (amb_cog_layout): level 0 first."""
+    n = C.c_int32(0)
+    lw, lh = (C.c_int32 * 32)(), (C.c_int32 * 32)()
+    st = _lib.lib().amb_cog_layout(int(width), int(height), int(tile), C.byref(n), lw, lh)
+    if st != _lib.AMB_OK:
+        raise ValueError("no COG levels for a %r x %r raster in tiles of %r" % (width, height, tile))
+    return [(lw[k], lh[k]) for k in range(n.value)]
+
+
+def cog_nodata(fmt, nodata):
+    """The GDAL_NODATA written for `nodata`, which must agree with the overviews' reduction: NaN for "f32" (NaN pixels
+    are left out of the means), 0 for "mask8" (the maximum keeps 0 only where every child is 0), none for "gray8" and
+    "bgr8" (their means would take a no-data value in).  Anything else raises ValueError."""
+    if nodata is None:
+        return None
+    if fmt == "f32":
+        if isinstance(nodata, str) and nodata.strip().lower() == "nan":
+            return "nan"
+        if isinstance(nodata, (float, np.floating)) and math.isnan(nodata):
+            return "nan"
+    elif fmt == "mask8":
+        if not isinstance(nodata, (str, bool, np.bool_)) and isinstance(nodata, (int, float, np.integer, np.floating)) \
+                and nodata == 0:
+            return 0
+    raise ValueError("COG nodata %r does not agree with the %r overviews: use %s" % (
+        nodata, fmt, {"f32": "'nan'", "mask8": "0"}.get(fmt, "None")))
+
+
+def write_cog(path, data, tile_bytes, width, height, fmt, tile, geotransform, epsg=32632, nodata=None):
+    """Writes Cloud-Optimized GeoTIFF tiles (GridMap.to_cog, cog_tiles; convention in include/aerial_mapper_b200.h,
+    amb_cog_tiles_device) as a classic TIFF: the header, the IFD of level 0 at offset 8 and then those of the overviews
+    in decreasing size, each followed by its out-of-line values, then the tile data in file order (the smallest level
+    first, row-major within a level).  Every IFD has TileWidth = TileLength = tile, Compression 8 and the predictor of
+    write_geotiff_strips; level 0 has NewSubfileType 0 and the georeferencing and GDAL_NODATA, each overview
+    NewSubfileType 1.  nodata: see cog_nodata.  data: the tiles back to back; tile_bytes: each tile's length.  A file
+    over 4 GiB raises ValueError (no BigTIFF)."""
+    bands, bits, predictor = _DEFLATE_FORMATS[fmt]
+    nd = cog_nodata(fmt, nodata)
+    gt = _north_up(geotransform)
+    data = memoryview(data).cast("B")
+    counts = [int(v) for v in tile_bytes]
+    levels = cog_layout(width, height, tile)
+    n_tiles = [-(-w // tile) * -(-h // tile) for w, h in levels]
+    if len(counts) != sum(n_tiles) or sum(counts) != len(data):
+        raise ValueError("write_cog: %d tiles of %d bytes in all do not fit a %d x %d raster in tiles of %d (%d tiles)"
+                         % (len(counts), sum(counts), width, height, tile, sum(n_tiles)))
+    first = np.cumsum([0] + n_tiles[::-1])[::-1][1:]      # each level's first tile in file order (the smallest first)
+    tags = []
+    for k, (w, h) in enumerate(levels):
+        c = counts[first[k]:first[k] + n_tiles[k]]
+        layout = [(322, _LONG, [tile]), (323, _LONG, [tile]), (324, _LONG, [0] * len(c)), (325, _LONG, c)]
+        tags.append(_image_tags(w, h, bands, bits, predictor, layout, (gt, epsg, nd) if k == 0 else None,
+                                subfile=0 if k == 0 else 1))
+    ifd_at = [8]
+    for t in tags:
+        ifd_at.append(ifd_at[-1] + _ifd_size(t))
+    data_at = (ifd_at[-1] + 15) & ~15
+    _check_size(data_at + len(data))
+    starts = np.concatenate([[0], np.cumsum(np.asarray(counts, np.int64))[:-1]]) + data_at
+    head = b"II*\0" + struct.pack("<I", 8)
+    for k, t in enumerate(tags):
+        t = _set_tag(t, 324, _LONG, [int(v) for v in starts[first[k]:first[k] + n_tiles[k]]])
+        head += _ifd(t, ifd_at[k], ifd_at[k + 1] if k + 1 < len(tags) else 0)
+    with open(path, "wb") as f:
+        f.write(head + b"\0" * (data_at - len(head)))
         f.write(data)
 
 
@@ -301,8 +405,9 @@ def _unsupported(tag, value, why):
     raise ValueError("read_geotiff: %s = %r is not supported (%s)" % (tag, value, why))
 
 
-def _read_ifd(data):
-    """Tag -> tuple of values (ASCII: str) of the first IFD of a classic little-endian TIFF."""
+def _read_ifd(data, at=None):
+    """Tag -> tuple of values (ASCII: str) of the IFD at offset `at` (by default the first) of a classic little-endian
+    TIFF."""
     if len(data) < 8:
         raise ValueError("read_geotiff: not a TIFF file (%d bytes)" % len(data))
     if data[:2] == b"MM":
@@ -314,7 +419,8 @@ def _read_ifd(data):
         _unsupported("version", 43, "BigTIFF")
     if magic != 42:
         raise ValueError("read_geotiff: not a TIFF file (version %d)" % magic)
-    at = struct.unpack_from("<I", data, 4)[0]
+    if at is None:
+        at = struct.unpack_from("<I", data, 4)[0]
     n = struct.unpack_from("<H", data, at)[0]
     tags = {}
     for e in range(n):
@@ -329,6 +435,28 @@ def _read_ifd(data):
         else:
             tags[tag] = struct.unpack_from("<%d%s" % (count * len(fmt), fmt[0]), buf)
     return tags
+
+
+def _next_ifd(data, at):
+    """The offset of the IFD after the one at `at` (0: none)."""
+    return struct.unpack_from("<I", data, at + 2 + 12 * struct.unpack_from("<H", data, at)[0])[0]
+
+
+def _overview_ifd(data, k):
+    """The IFD of overview k >= 1: the k-th IFD after the first that is a reduced image (NewSubfileType bit 0) and not a
+    mask (bit 2)."""
+    first = struct.unpack_from("<I", data, 4)[0]
+    seen, at, found = {first}, _next_ifd(data, first), 0
+    while at and at not in seen and at + 2 <= len(data):
+        seen.add(at)
+        tags = _read_ifd(data, at)
+        kind = tags.get(254, (0,))[0]
+        if kind & 1 and not kind & 4:
+            found += 1
+            if found == k:
+                return tags
+        at = _next_ifd(data, at)
+    raise ValueError("read_geotiff: overview %d requested, the file has %d" % (k, found))
 
 
 def _geotransform(tags):
@@ -383,7 +511,7 @@ def _undo_predictor(chunk, predictor, dtype, rows, cols, spp):
     return a
 
 
-def read_geotiff(path, band=0):
+def read_geotiff(path, band=0, overview=0):
     """A band of a GeoTIFF as GDAL writes DEMs: (array [H, W] in the file's sample type, GDAL geotransform (west, res_x, 0,
     north, 0, -res_y), EPSG code or None, no-data value or None).
 
@@ -394,11 +522,19 @@ def read_geotiff(path, band=0):
     EPSG: ProjectedCSTypeGeoKey, else GeographicTypeGeoKey.  No-data: GDAL_NODATA as a float ("nan" included).  Anything
     else raises ValueError naming the tag and value (BigTIFF, big-endian, LZW, JPEG, rotated transforms ...).
 
+    overview k >= 1 reads the k-th reduced-resolution IFD after the first (a COG's levels, GridMap.to_cog), whose
+    geotransform is the first IFD's with its pixel sizes scaled by W / w_k and H / h_k (GDAL's rule); EPSG and no-data
+    are the first IFD's.  An overview the file does not have raises ValueError.
+
     For GridMap.from_raster a DEM is converted with a.astype(np.float32), its no-data value passed along: that value must
     be exact in float32 (true of every int16 and uint16 value) or pixels holding it will not compare equal."""
     with open(path, "rb") as f:
         data = f.read()
-    tags = _read_ifd(data)
+    if isinstance(overview, bool) or not isinstance(overview, (int, np.integer)) or overview < 0:
+        raise ValueError("read_geotiff: overview must be a non-negative integer, got %r" % (overview,))
+    base = tags = _read_ifd(data)
+    if overview:
+        tags = _overview_ifd(data, int(overview))
     width, height = tags[256][0], tags[257][0]
     spp = tags.get(277, (1,))[0]
     planar = tags.get(284, (1,))[0]
@@ -439,8 +575,12 @@ def read_geotiff(path, band=0):
             chunk = zlib.decompress(chunk)
         a = _undo_predictor(chunk, predictor, dtype, rows, cols, spp)
         out[r0:r0 + rows, c0:c0 + cols] = a[:height - r0, :width - c0, band]
-    keys = _geokeys(tags)
+    keys = _geokeys(base)
     epsg = keys.get(3072, keys.get(2048))
-    nodata = tags.get(42113)
-    return out, _geotransform(tags), (None if epsg in (None, 0, 32767) else int(epsg)), \
+    nodata = base.get(42113)
+    gt = _geotransform(base)
+    if overview:
+        sx, sy = base[256][0] / width, base[257][0] / height
+        gt = (gt[0], gt[1] * sx, gt[2], gt[3], gt[4], gt[5] * sy)
+    return out, gt, (None if epsg in (None, 0, 32767) else int(epsg)), \
         (None if nodata is None else float(nodata.strip()))

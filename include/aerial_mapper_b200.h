@@ -557,6 +557,46 @@ int amb_deflate_strips_device(amb_ctx* ctx, const void* d_image, int32_t width, 
 int amb_export_deflate_strips(amb_ctx* ctx, int layer, int format, int32_t rows_per_strip, void* host_out,
                               size_t capacity, size_t* size, uint32_t* strip_bytes);
 
+/* ---- Cloud-Optimized GeoTIFF tiles ----
+ * Convention.  The tiles of a tiled, Deflate-compressed TIFF with internal overviews, for a raster in one of the export's
+ * formats (amb_raster_format), width x height pixels, and a tile side T: a multiple of 16 with 16 <= T <= 4096.
+ *   Levels: level 0 is the raster; level k + 1 is ceil(w_k / 2) x ceil(h_k / 2) (= ceil(W / 2^k), GDAL's size rule),
+ *     added while level k is wider or taller than T.  A raster that fits one tile has no overviews.
+ *   Reduction: level k + 1 from level k (not from level 0).  Pixel (y, x) reads the children (2y + a, 2x + b), a, b in
+ *     {0, 1}, that lie inside level k (1 or 2 of them on the last row or column of an odd size):
+ *       AMB_RASTER_F32: the children that are not NaN, summed in IEEE double in the order (0,0), (0,1), (1,0), (1,1)
+ *         (the first one is the sum's start, so -0 survives), every operation rounded, no FMA; the sum divided by their
+ *         count n and stored as (float).  A NaN result (n == 0, or +inf and -inf among the children) is stored as the
+ *         quiet NaN 0x7FC00000, so NaN payloads never reach an overview.
+ *       AMB_RASTER_GRAY8, AMB_RASTER_BGR8: per byte the rounded mean (sum + n / 2) / n in integers.
+ *       AMB_RASTER_MASK8: the maximum, so the mask pyramid of a layer is "not NaN" of its F32 pyramid.
+ *     This is the project's own box filter; it is not promised to equal any GDAL resampling.
+ *   Tiles: each level is cut into ceil(w / T) x ceil(h / T) tiles, row-major; every tile is T x T pixels, those outside
+ *     the level zero.  A tile is one zlib stream exactly as a strip of amb_deflate_strips_device (Predictor 3 for F32,
+ *     2 for the 8-bit formats, BGR8 stored as RGB), a tile row of T pixels being the predictor's row, so a tile is never
+ *     longer than n + 5 ceil(n / 65535) + 6 bytes for its n = T * T * bytes-per-pixel predicted bytes.
+ *   Order: the smallest level's tiles first, then each larger level's, row-major within a level: the order of the
+ *     tiles' data in the file.
+ * Errors: those of amb_deflate_strips_device, and a bad T returns AMB_ERR_INVALID_ARGUMENT; a pyramid of more than
+ * 2^31 - 1 tile rows in all AMB_ERR_UNSUPPORTED.  Neither writes anything. */
+/* Host arithmetic, no GPU: the levels of a width x height raster at tile side `tile`; n_levels <= 32 entries of level_w
+ * and level_h are written.  AMB_ERR_INVALID_ARGUMENT for a NULL pointer, width or height <= 0 or a bad tile side. */
+int amb_cog_layout(int32_t width, int32_t height, int32_t tile, int32_t* n_levels, int32_t* level_w, int32_t* level_h);
+/* Host arithmetic, no GPU: the sum of the tiles' bounds; 0 if the arguments are invalid or unsupported. */
+size_t amb_cog_max_size(int32_t width, int32_t height, int format, int32_t tile);
+/* Builds the pyramid, tiles it and compresses every tile on the device, for a raster valid on the context's device
+ * (8-bit formats at any byte alignment), ordered after earlier work on the context's stream.  Synchronous: on return the
+ * tiles are in host_out back to back in file order (*size bytes, pinned or pageable) and tile_bytes[] holds each tile's
+ * length in the same order.  If capacity < *size it returns AMB_ERR_SIZE_MISMATCH with the size needed in *size and
+ * writes nothing else.  Device scratch, kept by the context: the overview levels (about 1/3 of the raster), the stacked
+ * tiles (the levels with their edge tiles padded) and the Deflate encoder's scratch for the stacked tiles. */
+int amb_cog_tiles_device(amb_ctx* ctx, const void* d_image, int32_t width, int32_t height, size_t row_stride,
+                         int format, int32_t tile, void* host_out, size_t capacity, size_t* size, uint32_t* tile_bytes);
+/* amb_export_raster_device of `layer` in `format` into the context's scratch, then amb_cog_tiles_device of it: the
+ * context's band (image rows [col_begin, col_end)) as an image of its own. */
+int amb_export_cog_tiles(amb_ctx* ctx, int layer, int format, int32_t tile, void* host_out, size_t capacity,
+                         size_t* size, uint32_t* tile_bytes);
+
 /* ---- measurement ---- */
 int amb_get_timings(amb_ctx* ctx, amb_timings* out);
 
