@@ -44,7 +44,7 @@
 
 namespace amb {
 
-using namespace dsmk;  // DsmPlan, PointRec, cell_x/cell_y, fine_bin, fast_rcp
+using namespace dsmk;  // DsmPlan, PointRec, cell_x/cell_y, fine_bin
 
 std::vector<double> dsm_thresholds(int32_t interpolation_radius) {
   // dsm.cc:133-144: lambda = 1; while (empty) { search(lambda*radius); lambda *= 1.1; if (lambda*radius > 7) break; }
@@ -543,10 +543,15 @@ __global__ void __launch_bounds__(256) dsm_cell_kernel(const __grid_constant__ D
         if (d2 < thr) {
           const double pz = __ldg(reinterpret_cast<const double*>(pr) + 2);
           ++cnt;
-          if (d2 > 0.0) {
+          if (d2 >= DBL_MIN) {   // (and < thr: inside fast_rcp's domain)
             const double w = fast_rcp(d2);
             num = fma(pz, w, num);
             den += w;
+          } else if (d2 > 0.0) {
+            // subnormal d2 (a point within ~1e-154 of the centre): the reference's own divisions, since z / d2 can
+            // stay finite where z * (1 / d2) overflows (dsm.cc:166-167, ortho-from-pcl.cc:99-100)
+            num += pz / d2;
+            den += 1.0 / d2;
           } else {
             coincident = true;
             const long long id = static_cast<long long>(rec_id(__ldg(&pr->idx)));

@@ -9,6 +9,7 @@
 #include <cfloat>
 #include <cstddef>
 
+#include "approx_math.h"
 #include "halo_push.h"
 namespace amb {
 namespace dsmk {
@@ -111,21 +112,6 @@ __device__ __forceinline__ double window_min_d2(const DsmPlan& p, const unsigned
 // of `list` in lane order.
 __device__ __forceinline__ void warp_append(bool take, unsigned int* counter, unsigned int* list, unsigned int value) {
   warp_reserve(take, counter, [&](unsigned int slot) { list[slot] = value; });
-}
-
-// Reciprocal of a positive normal double to ~1 ulp: MUFU.RCP64H seed (rcp.approx.ftz.f64) + one cubic correction
-// step.  Replaces the two IEEE divisions per neighbour of the reference (heights/d2 and 1/d2) by one reciprocal
-// and one FMA; the IDW height changes by O(1e-16) relative, far inside the float32 layer's rounding.
-__device__ __forceinline__ double fast_rcp(double x) {
-  double r;
-#ifdef AMB_CUDA_EMU  // tests/emu (CPU emulation of the kernel source): no MUFU — an exact seed, same correction
-  r = 1.0 / x;
-#else
-  asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(r) : "d"(x));
-#endif
-  const double e = fma(-x, r, 1.0);  // |e| <= 2^-20
-  const double t = fma(e, e, e);     // e + e^2: r*(1 + e + e^2) leaves a relative error e^3 <= 2^-60
-  return fma(r, t, r);
 }
 
 }  // namespace dsmk

@@ -19,6 +19,7 @@
 #include <mutex>
 
 #include "amb_context.h"
+#include "approx_math.h"
 
 namespace amb {
 namespace {
@@ -199,19 +200,6 @@ __device__ __noinline__ double exact_observation_angle(double xc, double yc, dou
   // u.norm() (:175) = sqrt(x*x + y*y + z*z), then asin(fabs(u(2)) / norm_u) (:177)
   const double n = sqrt(__dadd_rn(__dadd_rn(__dmul_rn(xc, xc), __dmul_rn(yc, yc)), __dmul_rn(zc, zc)));
   return asin(__ddiv_rn(fabs(zc), n));
-}
-
-// Reciprocal of a positive normal double to ~1 ulp: MUFU.RCP64H seed + one cubic correction step.
-__device__ __forceinline__ double fast_rcp(double x) {
-  double r;
-#ifdef AMB_CUDA_EMU  // tests/emu (CPU emulation of the kernel source): no MUFU — an exact seed, same correction
-  r = 1.0 / x;
-#else
-  asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(r) : "d"(x));
-#endif
-  const double e = fma(-x, r, 1.0);
-  const double t = fma(e, e, e);
-  return fma(r, t, r);
 }
 
 // aslam::PinholeCamera::project3: rz = 1/z; (u,v) = (x,y)*rz; distort; k = f*u + c.  Returns the reference's
