@@ -286,6 +286,8 @@ int amb_create(const amb_geometry* geom, int device, int32_t col_begin, int32_t 
 #endif
   if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking);
   if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking);
+  if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&ctx->scatter_stream, cudaStreamNonBlocking);
+  if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->scatter_start, cudaEventDisableTiming);
   for (int k = 0; k < EV_COUNT && e == cudaSuccess; ++k) e = cudaEventCreate(&ctx->events[k]);
   for (int k = 0; k < 2 && e == cudaSuccess; ++k) e = cudaEventCreateWithFlags(&ctx->copy_done[k], cudaEventDisableTiming);
   if (e != cudaSuccess) {
@@ -301,6 +303,7 @@ void amb_destroy(amb_ctx* ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
   if (ctx->stream) cudaStreamSynchronize(ctx->stream);
+  if (ctx->scatter_stream) cudaStreamSynchronize(ctx->scatter_stream);  // (joined by `stream` unless a DSM call failed)
   amb_comm_destroy(ctx);
   ctx->halo_send.release();
   ctx->halo_recv.release();
@@ -314,6 +317,8 @@ void amb_destroy(amb_ctx* ctx) {
   for (DeviceBuffer* b : bufs) b->release();
   for (int k = 0; k < EV_COUNT; ++k)
     if (ctx->events[k]) cudaEventDestroy(ctx->events[k]);
+  if (ctx->scatter_start) cudaEventDestroy(ctx->scatter_start);
+  for (cudaEvent_t e : ctx->band_done) cudaEventDestroy(e);
   for (int k = 0; k < 2; ++k)
     if (ctx->copy_done[k]) cudaEventDestroy(ctx->copy_done[k]);
   for (int l = 0; l < AMB_NUM_LAYERS; ++l)
@@ -326,6 +331,7 @@ void amb_destroy(amb_ctx* ctx) {
   if (ctx->host_flags) cudaFreeHost(ctx->host_flags);
   if (ctx->stream) cudaStreamDestroy(ctx->stream);
   if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
+  if (ctx->scatter_stream) cudaStreamDestroy(ctx->scatter_stream);
   delete ctx;
 }
 

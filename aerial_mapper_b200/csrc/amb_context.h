@@ -139,6 +139,11 @@ struct amb_ctx {
   int32_t col_begin = 0, col_end = 0;  // owned column stripe
   cudaStream_t stream = nullptr;
   cudaStream_t copy_stream = nullptr;  // H2D staging overlapped with compute
+  // the DSM binning's fine scatter, one launch per band of bucket columns, overlapped with the gather on `stream`
+  // (dsm_run): it waits for scatter_start, and the gather of the tile columns over band d waits for band_done[d]
+  cudaStream_t scatter_stream = nullptr;
+  cudaEvent_t scatter_start = nullptr;
+  std::vector<cudaEvent_t> band_done;  // grown to the most bands a binning used
   cudaEvent_t events[amb::EV_COUNT] = {};
   cudaEvent_t copy_done[2] = {};
   // pinned staging of per-call tables, double-buffered: call k fills stages[k & 1] while the asynchronous copies and the
@@ -286,5 +291,11 @@ int sharded_step(amb_ctx* ctx, const double* d_xyz, const int* d_intensities, co
                  int mode);
 std::vector<double> dsm_thresholds(int32_t interpolation_radius);
 double dsm_tile_reach_cells(double resolution, int32_t interpolation_radius);  // tile width + window apron + 1, in cells
+namespace dsmk {
+struct DsmPlan;
+}
+// The band of the binning's fine scatter (bucket columns kj with kj / kj_per == band) that the reads of a tile column
+// (global tile index `tile`) wait for, when they reach `reach` cells past the tile (W: the gather; P: the fill)
+int dsm_scatter_band(const dsmk::DsmPlan& plan, int kj_per, int tile, int reach);
 
 }  // namespace amb

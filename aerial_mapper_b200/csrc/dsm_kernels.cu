@@ -14,11 +14,13 @@
 //   SMEM:  a 32x32-cell tile loads the buckets overlapping its window (tile + apron), bins their points with
 //          shared-memory atomics, orders every bin's points by original index, and gathers from there.
 //
-// Pipeline (all on the context's stream):
+// Pipeline (on the context's stream, except K3):
 //   K1 dsm_partition_kernel      (dsm_partition.inc) bins every point once in double precision, counts the buckets
 //                                (atomics resolve in L2) and groups each tile of 2048 points by coarse destination
 //   K2 scan_*                    inclusive scan of the bucket counts -> bucket start offsets
-//   K3 dsm_fine_scatter_kernel   (dsm_partition.inc) records into bucket order, one coarse destination at a time
+//   K3 dsm_fine_scatter_kernel   (dsm_partition.inc) records into bucket order, one launch per coarse destination (a
+//                                band of bucket columns) on the context's scatter stream; K4 for the tile columns over
+//                                band d waits for band d only, so it runs while the later bands are scattered
 //   K4 dsm_gather_kernel_f32     one tile per block: bucket runs -> bins in shared memory -> every thread owns a 1x4
 //      dsm_gather_kernel         strip of cells and walks the strip's bin rows in one flattened loop.  FP32 sums with
 //                                exact decisions (the default; Dsm only) or all FP64; cells it cannot decide exactly
@@ -29,7 +31,7 @@
 //                                of atomic scheduling and of how the map is striped across GPUs)
 //   K6 dsm_cell_kernel           one warp per listed cell: the expanding-radius retry (dsm.cc:133-144) and the cells
 //                                handed over by K4, from the bucket records in HBM
-// With amb_dsm_set_stream_chunks, K4-K6 run once per group of tile columns.
+// With amb_dsm_set_stream_chunks, K4-K6 run once per group of tile columns.  K5 and K6 start once K3 is done.
 //
 // Membership (d2 < threshold) is evaluated with __dmul_rn/__dadd_rn (no FMA contraction) in the reference's
 // operation order, so neighbour sets and retry levels are bit-exact decisions.  Heights differ from the CPU only
@@ -66,6 +68,7 @@ constexpr int kGatherThreads = 256;
 constexpr int kStrip = 4;           // cells per thread in the gather kernel (adjacent along j)
 constexpr int kScanChunk = 4096;    // elements per block in the scan kernels (256 threads x 16)
 constexpr int kSortRegs = 4;        // bucket sort: records per lane held in registers (buckets up to 128 points)
+constexpr int kScatterBlocksPerSm = 1;  // P2's grid while the gather runs beside it (dsm_run)
 static_assert(TJ == kStrip * (kGatherThreads / 32), "one warp per strip row of the tile");
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -602,6 +605,15 @@ double dsm_tile_reach_cells(double resolution, int32_t interpolation_radius) {
   return static_cast<double>(TJ + W + 1);
 }
 
+// A tile column's reads within `reach` cells (gather_tile, bucket_window) cover bucket columns up to that of its last
+// cell + reach, and they read G[kj * KR + kbi0] .. G[kj * KR + kbi1 + 1] over them.  After P2, G[b] is bucket b - 1's
+// cursor, so the first of these entries can belong to the bucket column before the first one: an earlier band, which the
+// scatter stream, running in band order, has finished before the band of the last bucket column.
+int dsm_scatter_band(const DsmPlan& plan, int kj_per, int tile, int reach) {
+  const int last_bin = std::min((tile + 1) * TJ - 1 - plan.gj0 + reach, plan.BC - 1);
+  return (last_bin >> plan.Bshift) / kj_per;
+}
+
 namespace {
 
 // Half-width (in bins along i) of the window that can hold a point with d2 < thr, for a bin row |dj| away.
@@ -783,6 +795,9 @@ int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, 
   unsigned int* counters = ctx->counters.as<unsigned int>();
   PointRec* rec = ctx->records.as<PointRec>();
 
+  // a call that failed between its scatter and its join left the scatter stream running into the bins
+  if (ctx->last_bin_destinations > 0)
+    AMB_CUDA(ctx, cudaStreamWaitEvent(s, ctx->band_done[ctx->last_bin_destinations - 1], 0));
   // the bins are rewritten from here on: until this call stores its plan they describe no plan
   ctx->last_dsm_plan.clear();
   ctx->last_bin_destinations = 0;
@@ -806,8 +821,9 @@ int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, 
   pp.halo_base = halo ? ((n_own + kPartTile - 1) / kPartTile) * kPartTile : n_own;   // halo slots start a new tile
   pp.n_total = n;
   // a destination = a band of bucket columns whose final records span ~48 MB at a uniform density, about the H100's
-  // 50 MB L2; at most kMaxCoarse bands.  Measured on an H100 SXM (80 GB, 400 W power limit) at 50 M points, whole binning
-  // stage: 48 MB 4.69 ms, 32 MB 4.77 ms, 24 MB 4.87 ms, 16 MB 4.92 ms
+  // 50 MB L2; at most kMaxCoarse bands.  Measured on an H100 SXM (80 GB, 700 W power limit) at 50 M points, P2 and the
+  // gather beside it (DESIGN §4.0): 48 MB 5.01 ms, 32 MB 5.19 ms, 24 MB 5.48 ms, 16 MB 5.72 ms, 64 MB 4.96 ms (within the
+  // 48 MB runs' spread, and past the L2 that P2 on its own relies on)
   // (test knob AMB_DSM_PART_WINDOW: bytes per destination — small values exercise many destinations on small maps)
   static const size_t window_bytes = [] {
     const char* e = std::getenv("AMB_DSM_PART_WINDOW");
@@ -861,18 +877,44 @@ int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, 
   scan_spine_kernel<<<1, 1024, 0, s>>>(ctx->block_sums.as<unsigned int>(), scan_blocks);
   scan_apply_kernel<<<scan_blocks, 256, 0, s>>>(reinterpret_cast<uint4*>(G), n_vec,
                                                 ctx->block_sums.as<unsigned int>());
-  dsm_fine_scatter_kernel<<<static_cast<unsigned int>(pp.S) * pp.n_groups, kFineThreads, 0, s>>>(
-      plan, pp, ctx->records_tmp.as<PointRec>(), ctx->tile_offsets.as<unsigned short>(), G, rec);
+  if (!whole_map_bins) AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_BIN_END], s));
+  // P2 on the scatter stream, one launch per band of bucket columns, each followed by its band_done event: the gather of
+  // the tile columns over band d (on `s`, below) waits for band_done[d] only, so it runs while the later bands are
+  // scattered.  P2 is bound by HBM with few instructions per byte, the gather by instruction issue and shared memory.
+  // While a gather overlaps, P2's grid is one block per SM (kScatterBlocksPerSm): on an H100 SXM at C2 the two together
+  // took 4.99 ms with 1 block per SM, 5.09 ms with 2, 5.59 ms with 4 and 5.70 ms with P2's whole grid, against 5.73 ms
+  // one after the other (DESIGN §4.0); a higher priority for the scatter stream changed nothing measurable.  The paths
+  // that need every bucket before their next step (OrthoFromPcl's ordering of all buckets, whole_map_bins) join at once
+  // and give P2 its whole grid.
+  while (ctx->band_done.size() < static_cast<size_t>(pp.S)) {
+    cudaEvent_t e = nullptr;
+    AMB_CUDA(ctx, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    ctx->band_done.push_back(e);
+  }
+  cudaStream_t ss = ctx->scatter_stream;
+  AMB_CUDA(ctx, cudaEventRecord(ctx->scatter_start, s));
+  AMB_CUDA(ctx, cudaStreamWaitEvent(ss, ctx->scatter_start, 0));
+  const bool overlap = mode == 0 && !whole_map_bins;
+  const unsigned int scatter_grid =
+      overlap ? std::min(pp.n_groups, static_cast<unsigned int>(ctx->num_sms * kScatterBlocksPerSm)) : pp.n_groups;
+  for (int d = 0; d < pp.S; ++d) {
+    dsm_fine_scatter_kernel<<<scatter_grid, kFineThreads, 0, ss>>>(plan, pp, static_cast<unsigned int>(d),
+                                                                    ctx->records_tmp.as<PointRec>(),
+                                                                    ctx->tile_offsets.as<unsigned short>(), G, rec);
+    AMB_CUDA(ctx, cudaEventRecord(ctx->band_done[d], ss));
+  }
+  cudaEvent_t const scatter_end = ctx->band_done[pp.S - 1];
   ctx->last_bin_destinations = pp.S;
+  ctx->dsm_launches += 4 + pp.S;
   // Canonical order inside the buckets: Dsm orders only the buckets its warp-per-cell kernel will read (marked from the
   // cell list after the gather); OrthoFromPcl's adaptive pass may read any bucket, so that mode orders all of them here.
   unsigned char* bucket_flags = ctx->bucket_flags.as<unsigned char>();
+  if (!overlap) AMB_CUDA(ctx, cudaStreamWaitEvent(s, scatter_end, 0));
   if (mode == 1) {
     dsm_bucket_order_kernel<<<stream_grid, 256, 0, s>>>(G, static_cast<unsigned int>(nbk), rec,
                                                         ctx->point_order.as<unsigned int>(), nullptr);
     ctx->dsm_launches += 1;
   }
-  ctx->dsm_launches += 5;
   if (whole_map_bins) {
     AMB_CUDA(ctx, cudaGetLastError());
     plan.col_begin = ctx->col_begin;
@@ -881,7 +923,6 @@ int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, 
                               reinterpret_cast<const unsigned char*>(&plan) + sizeof(plan));
     return AMB_OK;
   }
-  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_BIN_END], s));
 
   // gather
   // FP32 gather (the default; amb_dsm_set_precision): Dsm only — OrthoFromPcl keeps the all-FP64 kernel
@@ -942,6 +983,9 @@ int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, 
   // the un-chunked ones restricted to its tile columns (plan.tile_j0 and the grid size), so every result is unchanged.
   // (Dsm only: OrthoFromPcl's adaptive pass rewrites the layer afterwards, so its columns are not final per chunk)
   // Without chunking the whole stripe is one group.
+  // Inside a group the gather is launched once per run of tile columns that wait for the same band of the scatter
+  // (dsm_scatter_band with the window's reach W); the fill waits for the band its reach P needs, which for the last
+  // group is the last band.
   const int chunks = (mode == 0 && ctx->dsm_stream_chunks > 1 && ctx->host_mirror[out_layer])
                          ? std::min(ctx->dsm_stream_chunks, tiles_j) : 1;
   for (int c = 0; c < chunks; ++c) {
@@ -949,9 +993,19 @@ int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, 
     const int tj1 = static_cast<int>(static_cast<long long>(tiles_j) * (c + 1) / chunks);
     if (tj1 <= tj0) continue;
     DsmPlan pc = plan;
-    pc.tile_j0 = plan.tile_j0 + tj0;
     if (c > 0) roll_list_counter_kernel<<<1, 1, 0, s>>>(counters);  // the cell list restarts; its length is kept
-    gather<<<ga.tiles_i * (tj1 - tj0), kGatherThreads, smem, s>>>(pc, ga);
+    for (int a = tj0; a < tj1;) {
+      const int band = dsm_scatter_band(plan, pp.kj_per, plan.tile_j0 + a, plan.W);
+      int b = a + 1;
+      while (b < tj1 && dsm_scatter_band(plan, pp.kj_per, plan.tile_j0 + b, plan.W) == band) ++b;
+      AMB_CUDA(ctx, cudaStreamWaitEvent(s, ctx->band_done[band], 0));
+      pc.tile_j0 = plan.tile_j0 + a;
+      gather<<<ga.tiles_i * (b - a), kGatherThreads, smem, s>>>(pc, ga);
+      ctx->dsm_launches += 1;
+      a = b;
+    }
+    const int fill_band = dsm_scatter_band(plan, pp.kj_per, plan.tile_j0 + tj1 - 1, plan.P);
+    AMB_CUDA(ctx, cudaStreamWaitEvent(s, ctx->band_done[fill_band], 0));
     if (chunks == 1) AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_GATHER_END], s));
     if (mode == 0) {
       dsm_mark_buckets_kernel<<<ctx->num_sms * 2, 256, 0, s>>>(pc, ga.cell_list, counters, bucket_flags);
@@ -960,7 +1014,7 @@ int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, 
       ctx->dsm_launches += 2;
     }
     dsm_cell_kernel<<<ctx->num_sms * 8, 256, 0, s>>>(pc, ca);
-    ctx->dsm_launches += 2;
+    ctx->dsm_launches += 1;
     if (chunks > 1) {
       // slab-local columns of this group's tiles (tiles are aligned to GLOBAL columns)
       const int col0 = std::max((plan.tile_j0 + tj0) * TJ - ctx->col_begin, 0);
@@ -971,6 +1025,8 @@ int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, 
   }
   // chunked: the stage split is not meaningful, both events mark the end
   if (chunks > 1) AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_GATHER_END], s));
+  // the join (the last group's fill has waited for the last band already): whatever follows on `s` finds the bins final
+  AMB_CUDA(ctx, cudaStreamWaitEvent(s, scatter_end, 0));
   AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_DSM_FILL_END], s));
   AMB_CUDA(ctx, cudaGetLastError());
   if (chunks == 1) {

@@ -97,8 +97,9 @@ typedef struct amb_camera {
 /* Device-side stage timings of the last process call, CUDA events on the context's stream (milliseconds). */
 typedef struct amb_timings {
   float dsm_h2d_ms;      /* host->device copy of the points (host entry point only) */
-  float dsm_bin_ms;      /* bin count + scan + scatter + in-bin canonical ordering */
-  float dsm_gather_ms;   /* tile IDW gather kernel (the dominant DSM kernel) */
+  float dsm_bin_ms;      /* bin count + scan */
+  float dsm_gather_ms;   /* scatter into the bins and the tile IDW gather (the dominant DSM kernel), which run at the
+                            same time (+ OrthoFromPcl's in-bin canonical ordering) */
   float dsm_fill_ms;     /* expanding-radius hole fill kernel */
   float dsm_total_ms;
   float ortho_h2d_ms;    /* host->device copy of the needed frame sub-rectangles (host entry point only) */

@@ -12,8 +12,10 @@ HBM).  Two runs in one process:
      memsets          the bucket counts G (4 B per bucket) + the bucket flags (1 B per bucket) + the stage counters
      P1 partition     24 B read + 32 B written per point, + the uint16 run-start table
      scan_reduce      G read once;  scan_apply: G read and written;  scan_spine: the block sums
-     P2 fine_scatter  32 B read + 32 B written per point, + the run-start table read
-   plus the stage's span on the device (first memset start -> P2 end), which includes the launch gaps.
+     P2 fine_scatter  32 B read + 32 B written per point, + the run-start table read (summed over its launches, one
+                      per band)
+   plus the stage's span on the device (first memset start -> last P2 end), which includes the launch gaps and, since
+   the gather runs beside P2 (tools/overlap_trace.py), part of the gather.
 
 Prints the card's name and power limit, one JSON line per copy, one per kernel and one for the stage.
 """
@@ -134,7 +136,7 @@ def kernel_key(name):
 
 
 def split_stage(events):
-    """Per binning call: device ms per kernel kind, and the stage span (first memset start -> P2 end)."""
+    """Per binning call: device ms per kernel kind, and the stage span (first memset start -> last P2 end)."""
     dev = sorted((ev for ev in map(_ev, events) if ev[3]), key=lambda ev: ev[1])
     calls = []
     for i, (name, start, dur, _) in enumerate(dev):
@@ -148,14 +150,14 @@ def split_stage(events):
             first = dev[j][1]
             j -= 1
         j = i
-        while j < len(dev):
+        while j < len(dev):   # P2 is one launch per band, interleaved with the gather: up to the next call's memsets
             k = kernel_key(dev[j][0])
-            if k is None or k == "memset":
+            if k == "memset" or (k == "dsm_partition_kernel" and j > i):
                 break
-            call[k] += dev[j][2] / 1e6
+            if k is not None:
+                call[k] += dev[j][2] / 1e6
             if k == "dsm_fine_scatter_kernel":
                 call["stage_span"] = (dev[j][1] + dev[j][2] - first) / 1e6
-                break
             j += 1
         if "stage_span" in call:
             calls.append(call)
