@@ -72,19 +72,50 @@ int ensure_counters(amb_ctx* ctx) {
   return AMB_OK;
 }
 
-int ensure_layer(amb_ctx* ctx, int layer) {
-  if (layer < 0 || layer >= AMB_NUM_LAYERS) return AMB_ERR_INVALID_ARGUMENT;
+// AerialGridMap's initial value of a layer (aerial-mapper-grid-map.cc:40-48)
+static float initial_value(int layer) {
+  if (layer == AMB_LAYER_ORTHO) return 255.0f;
+  if (layer == AMB_LAYER_ELEVATION_ANGLE || layer == AMB_LAYER_NUM_OBSERVATIONS) return 0.0f;
+  return std::numeric_limits<float>::quiet_NaN();
+}
+
+static int fill_layer(amb_ctx* ctx, int layer) {
+  wait_layer_copy(ctx, layer);
+  fill_kernel<<<ctx->num_sms * 4, 256, 0, ctx->stream>>>(ctx->layers[layer], ctx->slab_cells(), initial_value(layer));
+  AMB_CUDA(ctx, cudaGetLastError());
+  return AMB_OK;
+}
+
+static int alloc_layer(amb_ctx* ctx, int layer) {
   if (ctx->layers[layer]) return AMB_OK;
   AMB_CUDA(ctx, cudaSetDevice(ctx->device));
   float* p = nullptr;
   AMB_CUDA(ctx, cudaMalloc(&p, ctx->slab_cells() * sizeof(float)));
   ctx->layers[layer] = p;
-  // A layer that was never uploaded starts with AerialGridMap's initial value (aerial-mapper-grid-map.cc:40-48).
-  float v = std::numeric_limits<float>::quiet_NaN();
-  if (layer == AMB_LAYER_ORTHO) v = 255.0f;
-  if (layer == AMB_LAYER_ELEVATION_ANGLE || layer == AMB_LAYER_NUM_OBSERVATIONS) v = 0.0f;
-  fill_kernel<<<ctx->num_sms * 4, 256, 0, ctx->stream>>>(p, ctx->slab_cells(), v);
-  AMB_CUDA(ctx, cudaGetLastError());
+  ctx->layer_fresh[layer] = true;
+  return AMB_OK;
+}
+
+int ensure_layer(amb_ctx* ctx, int layer) {
+  if (layer < 0 || layer >= AMB_NUM_LAYERS) return AMB_ERR_INVALID_ARGUMENT;
+  const int st = alloc_layer(ctx, layer);
+  if (st != AMB_OK || !ctx->layer_fresh[layer]) return st;
+  ctx->layer_fresh[layer] = false;
+  return fill_layer(ctx, layer);
+}
+
+bool layer_is_fresh(const amb_ctx* ctx, int layer) {
+  return !ctx->eager_layer_init && (!ctx->layers[layer] || ctx->layer_fresh[layer]);
+}
+
+int ensure_layer_overwrite(amb_ctx* ctx, int layer, bool* fresh) {
+  if (layer < 0 || layer >= AMB_NUM_LAYERS) return AMB_ERR_INVALID_ARGUMENT;
+  *fresh = false;
+  if (ctx->eager_layer_init) return ensure_layer(ctx, layer);
+  const int st = alloc_layer(ctx, layer);
+  if (st != AMB_OK) return st;
+  *fresh = ctx->layer_fresh[layer];
+  ctx->layer_fresh[layer] = false;
   return AMB_OK;
 }
 
@@ -278,6 +309,8 @@ int amb_create(const amb_geometry* geom, int device, int32_t col_begin, int32_t 
     if (p[0] == 'f' && p[1] == '6') ctx->dsm_precision = AMB_DSM_F64;
     if (p[0] == 'f' && p[1] == '3') ctx->dsm_precision = AMB_DSM_F32;
   }
+  // A/B switch of the deferred reset (amb_init_layers): 1 fills every existing slab at once, as a separate pass
+  if (const char* p = std::getenv("AMB_EAGER_LAYER_INIT")) ctx->eager_layer_init = p[0] == '1';
   cudaError_t e = cudaSetDevice(device);
 #ifdef AMB_CUDA_EMU  // tests/emu (CPU emulation of the kernel source): grid-stride launches need no more blocks than this
   ctx->num_sms = 2;
@@ -368,25 +401,26 @@ void* amb_stream(amb_ctx* ctx) { return ctx ? static_cast<void*>(ctx->stream) : 
 int amb_init_layers(amb_ctx* ctx) {
   if (!ctx) return AMB_ERR_INVALID_ARGUMENT;
   AMB_CUDA(ctx, cudaSetDevice(ctx->device));
-  const float nan = std::numeric_limits<float>::quiet_NaN();
   for (int l = 0; l < AMB_NUM_LAYERS; ++l) {
-    // Slabs are allocated lazily and a fresh slab is born with its initial value (ensure_layer), so only the
-    // ones that already exist need refilling.
+    // Slabs are allocated lazily and start fresh, so only the ones that already exist need resetting.  The reset is
+    // deferred: the next ensure_layer fills the slab, and a writer of every cell (ensure_layer_overwrite) stores the
+    // initial values itself, which spares a pass over the slab.
     if (!ctx->layers[l]) continue;
     wait_layer_copy(ctx, l);
-    float v = nan;
-    if (l == AMB_LAYER_ORTHO) v = 255.0f;
-    if (l == AMB_LAYER_ELEVATION_ANGLE || l == AMB_LAYER_NUM_OBSERVATIONS) v = 0.0f;
-    fill_kernel<<<ctx->num_sms * 4, 256, 0, ctx->stream>>>(ctx->layers[l], ctx->slab_cells(), v);
+    ctx->layer_fresh[l] = true;
+    if (ctx->eager_layer_init) {
+      const int st = ensure_layer(ctx, l);
+      if (st != AMB_OK) return st;
+    }
   }
-  AMB_CUDA(ctx, cudaGetLastError());
   return AMB_OK;
 }
 
 int amb_upload_layer(amb_ctx* ctx, int layer, const float* host_slab) {
   if (!ctx || !host_slab) return AMB_ERR_INVALID_ARGUMENT;
   AMB_CUDA(ctx, cudaSetDevice(ctx->device));
-  int st = ensure_layer(ctx, layer);
+  bool fresh;  // the copy writes every cell
+  int st = ensure_layer_overwrite(ctx, layer, &fresh);
   if (st != AMB_OK) return st;
   wait_layer_copy(ctx, layer);
   st = staged_h2d(ctx, ctx->layers[layer], host_slab, ctx->slab_cells() * sizeof(float), ctx->stream);
@@ -398,7 +432,8 @@ int amb_upload_layer(amb_ctx* ctx, int layer, const float* host_slab) {
 int amb_upload_layer_device(amb_ctx* ctx, int layer, const float* device_slab) {
   if (!ctx || !device_slab) return AMB_ERR_INVALID_ARGUMENT;
   AMB_CUDA(ctx, cudaSetDevice(ctx->device));
-  int st = ensure_layer(ctx, layer);
+  bool fresh;  // the copy writes every cell
+  int st = ensure_layer_overwrite(ctx, layer, &fresh);
   if (st != AMB_OK) return st;
   wait_layer_copy(ctx, layer);
   AMB_CUDA(ctx, cudaMemcpyAsync(ctx->layers[layer], device_slab, ctx->slab_cells() * sizeof(float),

@@ -162,6 +162,11 @@ struct amb_ctx {
   std::string last_error;
 
   float* layers[AMB_NUM_LAYERS] = {};
+  // Deferred reset: amb_init_layers only marks an existing slab fresh; its initial value is written by the first
+  // ensure_layer (a fill) or, without a fill, by a writer that takes it through ensure_layer_overwrite.  A slab born in
+  // ensure_layer_overwrite starts fresh as well.  AMB_EAGER_LAYER_INIT=1 (read at amb_create) fills at once instead.
+  bool layer_fresh[AMB_NUM_LAYERS] = {};
+  bool eager_layer_init = false;
 
   // DSM scratch
   amb::DeviceBuffer points;       // device copy of the caller's xyz (host entry point)
@@ -244,7 +249,11 @@ inline int fail(amb_ctx* ctx, cudaError_t e, const char* what) {
   } while (0)
 
 int ensure_counters(amb_ctx* ctx);  // allocates (zeroed) the flag/counter block on first use
-int ensure_layer(amb_ctx* ctx, int layer);
+int ensure_layer(amb_ctx* ctx, int layer);  // allocates the slab, and writes its initial value while it is fresh
+// For a writer that stores EVERY cell of the slab: allocates the slab, returns in *fresh whether it still has to take
+// the initial value (then the writer stores it wherever it has no result of its own) and clears the flag.
+int ensure_layer_overwrite(amb_ctx* ctx, int layer, bool* fresh);
+bool layer_is_fresh(const amb_ctx* ctx, int layer);  // what ensure_layer_overwrite would return now
 int wait_layer_copy(amb_ctx* ctx, int layer);  // writers of a layer wait for its pending asynchronous download
 int enqueue_layer_download(amb_ctx* ctx, int layer, float* host_slab);  // on the copy stream, after current work
 int mirror_layer(amb_ctx* ctx, int layer);

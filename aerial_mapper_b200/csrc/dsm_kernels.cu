@@ -495,6 +495,7 @@ struct CellArgs {
   unsigned int* counters;
   int* dbg_count;
   signed char* dbg_level;
+  int fresh;  // the layer still has to take its initial value (ensure_layer_overwrite): NaN where no level reaches
 };
 
 __global__ void __launch_bounds__(256) dsm_cell_kernel(const __grid_constant__ DsmPlan plan, const CellArgs args) {
@@ -518,7 +519,8 @@ __global__ void __launch_bounds__(256) dsm_cell_kernel(const __grid_constant__ D
         break;
       }
     }
-    if (level < 0) {  // stays untouched (NaN or the previous elevation)
+    if (level < 0) {  // the previous elevation stays (dsm.cc:133-144); a fresh layer takes its initial NaN here
+      if (args.fresh && lane == 0) args.elevation[cell] = __int_as_float(0x7fc00000);
       if (args.dbg_count && lane == 0) {
         args.dbg_count[cell] = 0;
         args.dbg_level[cell] = -1;
@@ -710,9 +712,6 @@ int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, 
   if (halo) n = ((n_own + 2047) / 2048) * 2048 + static_cast<size_t>(halo->nranks) * halo->capacity;
   if (interpolation_radius < 1 || n >= size_t(0xffffffffu)) return AMB_ERR_INVALID_ARGUMENT;
   const int out_layer = mode == 1 ? AMB_LAYER_ORTHO : AMB_LAYER_ELEVATION;  // ortho-from-pcl.cc:51 / dsm.cc:116
-  int st = ensure_layer(ctx, out_layer);
-  if (st != AMB_OK) return st;
-  wait_layer_copy(ctx, out_layer);
 
   DsmPlan plan;
   std::memset(&plan, 0, sizeof(plan));
@@ -784,7 +783,7 @@ int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, 
   AMB_CUDA(ctx, ctx->point_order.reserve(n * sizeof(unsigned int)));
   AMB_CUDA(ctx, ctx->bucket_flags.reserve(nbk));
   AMB_CUDA(ctx, ctx->empty_cells.reserve(cells * sizeof(unsigned int)));
-  st = ensure_counters(ctx);
+  int st = ensure_counters(ctx);
   if (st != AMB_OK) return st;
   if (ctx->dsm_debug) {
     AMB_CUDA(ctx, ctx->dbg_count.reserve(cells * sizeof(int)));
@@ -955,6 +954,14 @@ int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, 
   smem = std::max(smem, off_bytes + per_point * 64);
   smem = (smem + 1023) & ~static_cast<size_t>(1023);
   const int capacity = static_cast<int>((smem - off_bytes) / per_point) & ~1;
+  // Dsm stores every cell of the stripe — the gather the cells it evaluates, the warp-per-cell kernel all the others
+  // (whole tiles handed over included), NaN where no retry level reaches a point — so a fresh elevation layer is not
+  // filled first.  OrthoFromPcl leaves a cell without a neighbour untouched: its layer is filled.  (Taken here, after
+  // the last check that can turn the call down, so that a refused call leaves the layer fresh.)
+  bool fresh = false;
+  st = mode == 0 ? ensure_layer_overwrite(ctx, out_layer, &fresh) : ensure_layer(ctx, out_layer);
+  if (st != AMB_OK) return st;
+  wait_layer_copy(ctx, out_layer);
   void (*const gather)(DsmPlan, GatherArgs) = f32 ? dsm_gather_kernel_f32 : dsm_gather_kernel;
   AMB_CUDA(ctx, cudaFuncSetAttribute(gather, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   GatherArgs ga;
@@ -976,6 +983,7 @@ int dsm_run(amb_ctx* ctx, const double* d_xyz, const unsigned long long* d_ids, 
   ca.counters = counters;
   ca.dbg_count = ga.dbg_count;
   ca.dbg_level = ga.dbg_level;
+  ca.fresh = fresh ? 1 : 0;
   const int tiles_j = tile_j1 - plan.tile_j0 + 1;
   // Opt-in chunking (amb_dsm_set_stream_chunks, only with a registered host mirror): the tile columns are evaluated in K
   // groups — gather + warp-per-cell fill per group — and each group's finished columns start travelling to the host

@@ -293,6 +293,22 @@ __device__ __forceinline__ void store_winner(const OrthoArgs& a, int* s_bbox, si
   }
 }
 
+// The initial values of the layers a cell's winner writes (AerialGridMap's, ensure_layer), for a cell no frame wins in a
+// FRESH launch
+__device__ __forceinline__ void store_initial(const OrthoArgs& a, size_t cell) {
+  a.elevation_angle[cell] = 0.0f;
+  a.observation_index[cell] = __int_as_float(0x7fc00000);
+  a.out_layer[cell] = a.colored ? __int_as_float(0x7fc00000) : 255.0f;
+}
+
+// ... for every cell of a thread's strip inside the slab (a tile that returns before its winner selection)
+__device__ __forceinline__ void store_initial_strip(const OrthoArgs& a, int i, int jl0) {
+  if (i >= a.rows) return;
+#pragma unroll
+  for (int m = 0; m < kOStrip; ++m)
+    if (jl0 + m < a.cols_slab) store_initial(a, static_cast<size_t>(jl0 + m) * a.rows + i);
+}
+
 // One block = one OTI x OTJ cell tile; one thread = a 1 x kOStrip strip of cells (same i, adjacent j): the
 // per-frame constants are fetched once per thread and serve four cells, and the tile's cull list is built once
 // for 1024 cells.
@@ -300,6 +316,10 @@ __device__ __forceinline__ void store_winner(const OrthoArgs& a, int* s_bbox, si
 // SELECT = true:  phase A of the host-frame path: no texel access at all; records the winner's pixel per cell and
 //                 the bounding box of the winners' pixels per frame, so that only those sub-rectangles of the
 //                 host frames have to cross PCIe (phase B: ortho_texel_kernel).
+// FRESH = true (fused kernel only): elevation_angle, observation_index and out_layer are fresh (ensure_layer_overwrite):
+//                 the running best starts at their known initial 0 without a load, and every cell of the tile that no
+//                 frame wins takes the layers' initial values (store_initial).  A template parameter: as a run-time flag
+//                 the extra stores doubled the spills of the other instances.
 //
 // The frame list is culled by conservative view cone / rectangle tests (unless a.do_cull == 0: brute force) and, with
 // a.dominance, by the per-tile DOMINANCE cull:
@@ -313,8 +333,9 @@ __device__ __forceinline__ void store_winner(const OrthoArgs& a, int* s_bbox, si
 //   against the state without f also wins against the state with f or loses to g afterwards.  Dropping f therefore
 //   changes no output bit (tools/ortho_dominance_study.py checks this against the oracle) and leaves ~1.2 instead of
 //   ~8.5 frames per tile at the benchmark geometry.
-template <int DIST, bool SELECT>
+template <int DIST, bool SELECT, bool FRESH>
 __global__ void __launch_bounds__(kOrthoThreads, AMB_OBPS) ortho_kernel_dom(const __grid_constant__ OrthoArgs a) {
+  static_assert(!(SELECT && FRESH), "SELECT writes no texel: the host-frame path never runs fresh");
   __shared__ unsigned short s_list[kMaxFramesPerLaunch];
   __shared__ int s_bbox[SELECT ? 4 * kMaxFramesPerLaunch : 4];
   __shared__ float s_red[2][kOrthoThreads / 32];
@@ -366,7 +387,10 @@ __global__ void __launch_bounds__(kOrthoThreads, AMB_OBPS) ortho_kernel_dom(cons
     zmin = fminf(zmin, s_red[0][w]);
     zmax = fmaxf(zmax, s_red[1][w]);
   }
-  if (zmin > zmax) return;  // no cell of this tile has an elevation
+  if (zmin > zmax) {  // no cell of this tile has an elevation
+    if (FRESH) store_initial_strip(a, i, jl0);
+    return;
+  }
 
   // bounding sphere of the tile's landmarks (cell centres x elevation range)
   const int i1 = min(i0 + OTI, a.rows) - 1, j1 = min(j0 + OTJ, a.cols_slab) - 1;
@@ -482,8 +506,14 @@ __global__ void __launch_bounds__(kOrthoThreads, AMB_OBPS) ortho_kernel_dom(cons
 #ifdef AMB_CUDA_EMU  // tests/emu only: how many frames the tile keeps (plain vs dominance cull)
   if (threadIdx.x == 0) emu::note(a.dominance ? "ortho_dom_list" : "ortho_list", n_list);
 #endif
-  if (n_list == 0) return;
-  if (!SELECT && !validmask) return;  // (SELECT: every thread reaches the block-wide bbox flush below)
+  if (n_list == 0) {
+    if (FRESH) store_initial_strip(a, i, jl0);
+    return;
+  }
+  if (!SELECT && !validmask) {  // (SELECT: every thread reaches the block-wide bbox flush below)
+    if (FRESH) store_initial_strip(a, i, jl0);
+    return;
+  }
 
   // ---- winner selection: the reference's recurrence  `alpha_f > (double)best_f32  =>  best_f32 = (float)alpha_f`
   // with alpha = asin(|z|/norm)  (ortho-backward-grid.cc:173-183), evaluated WITHOUT an asin per candidate.
@@ -506,7 +536,7 @@ __global__ void __launch_bounds__(kOrthoThreads, AMB_OBPS) ortho_kernel_dom(cons
     best_f[m] = -1;
     double ref2 = 4.0, band = 0.0;  // invalid cell: nothing can win
     if ((validmask >> m) & 1u) {
-      best[m] = a.elevation_angle[static_cast<size_t>(jl0 + m) * a.rows + i];
+      best[m] = FRESH ? 0.0f : a.elevation_angle[static_cast<size_t>(jl0 + m) * a.rows + i];
       if (best[m] > 0.0f) {
         const double sb = sin(static_cast<double>(best[m]));
         ref2 = sb * sb;
@@ -542,7 +572,10 @@ __global__ void __launch_bounds__(kOrthoThreads, AMB_OBPS) ortho_kernel_dom(cons
     const double cz = fma(fc.m[6], X, fc.t[2]);
 #pragma unroll
     for (int m = 0; m < kOStrip; ++m) {
-      if (!((validmask >> m) & 1u)) continue;   // no elevation / beyond the map edge: untouched, nothing is read
+      if (!((validmask >> m) & 1u)) {  // no elevation / beyond the map edge: untouched, nothing is read
+        if (FRESH && i < a.rows && jl0 + m < a.cols_slab) store_initial(a, static_cast<size_t>(jl0 + m) * a.rows + i);
+        continue;
+      }
       double xc = fma(fc.m[1], Y[m], fma(fc.m[2], Z[m], cx));
       double yc = fma(fc.m[4], Y[m], fma(fc.m[5], Z[m], cy));
       double zc = fma(fc.m[7], Y[m], fma(fc.m[8], Z[m], cz));
@@ -575,7 +608,10 @@ __global__ void __launch_bounds__(kOrthoThreads, AMB_OBPS) ortho_kernel_dom(cons
           }
         }
       }
-      if (!win) continue;
+      if (!win) {
+        if (FRESH) store_initial(a, static_cast<size_t>(jl0 + m) * a.rows + i);
+        continue;
+      }
       const size_t cell = static_cast<size_t>(jl0 + m) * a.rows + i;
       // the pixel is round(keypoint) (:186-193): within the guard of a half-integer (or for a cell that took the exact
       // path) the keypoint is recomputed with the reference's operation sequence
@@ -657,7 +693,7 @@ __global__ void __launch_bounds__(kOrthoThreads, AMB_OBPS) ortho_kernel_dom(cons
 #pragma unroll
     for (int m = 0; m < kOStrip; ++m) {  // unrolled: the per-cell arrays must stay in registers
       if (!((dirty >> m) & 1u)) continue;
-      float b = a.elevation_angle[static_cast<size_t>(jl0 + m) * a.rows + i];
+      float b = FRESH ? 0.0f : a.elevation_angle[static_cast<size_t>(jl0 + m) * a.rows + i];
       int bf = -1;
       for (int l = 0; l < n_list; ++l) {
         const int f = s_list[l];
@@ -679,7 +715,10 @@ __global__ void __launch_bounds__(kOrthoThreads, AMB_OBPS) ortho_kernel_dom(cons
 
 #pragma unroll
   for (int m = 0; m < kOStrip; ++m) {
-    if (best_f[m] < 0) continue;
+    if (best_f[m] < 0) {
+      if (FRESH && i < a.rows && jl0 + m < a.cols_slab) store_initial(a, static_cast<size_t>(jl0 + m) * a.rows + i);
+      continue;
+    }
     const size_t cell = static_cast<size_t>(jl0 + m) * a.rows + i;
     // the winner's camera coordinates and keypoint, recomputed (the reference projects a second time too, :186-188)
     double xc, yc, zc, kx, ky, rz;
@@ -719,13 +758,15 @@ __global__ void __launch_bounds__(kOrthoThreads, AMB_OBPS) ortho_kernel_dom(cons
   }
 }
 
-template <bool SELECT>
+template <bool SELECT, bool FRESH>
 void launch_ortho_kernel(const OrthoArgs& a, int grid, cudaStream_t s) {
   switch (a.dist_type) {
-    case AMB_DIST_RADTAN: ortho_kernel_dom<AMB_DIST_RADTAN, SELECT><<<grid, kOrthoThreads, 0, s>>>(a); break;
-    case AMB_DIST_EQUIDISTANT: ortho_kernel_dom<AMB_DIST_EQUIDISTANT, SELECT><<<grid, kOrthoThreads, 0, s>>>(a); break;
-    case AMB_DIST_FOV: ortho_kernel_dom<AMB_DIST_FOV, SELECT><<<grid, kOrthoThreads, 0, s>>>(a); break;
-    default: ortho_kernel_dom<AMB_DIST_NONE, SELECT><<<grid, kOrthoThreads, 0, s>>>(a);
+    case AMB_DIST_RADTAN: ortho_kernel_dom<AMB_DIST_RADTAN, SELECT, FRESH><<<grid, kOrthoThreads, 0, s>>>(a); break;
+    case AMB_DIST_EQUIDISTANT:
+      ortho_kernel_dom<AMB_DIST_EQUIDISTANT, SELECT, FRESH><<<grid, kOrthoThreads, 0, s>>>(a);
+      break;
+    case AMB_DIST_FOV: ortho_kernel_dom<AMB_DIST_FOV, SELECT, FRESH><<<grid, kOrthoThreads, 0, s>>>(a); break;
+    default: ortho_kernel_dom<AMB_DIST_NONE, SELECT, FRESH><<<grid, kOrthoThreads, 0, s>>>(a);
   }
 }
 
@@ -949,8 +990,14 @@ int ortho_run(amb_ctx* ctx, const amb_camera* camera, const double* T_G_B, const
   if (camera->dist_type < AMB_DIST_NONE || camera->dist_type > AMB_DIST_FOV) return AMB_ERR_UNSUPPORTED;
   const int out_layer = colored_ortho ? AMB_LAYER_COLORED_ORTHO : AMB_LAYER_ORTHO;
   const int need[4] = {AMB_LAYER_ELEVATION, AMB_LAYER_ELEVATION_ANGLE, AMB_LAYER_OBSERVATION_INDEX, out_layer};
+  // One fused launch (frames on the device, at most one chunk of them) writes every cell of the slab: when all three
+  // layers it writes are fresh, it stores their initial values itself instead of reading them after a fill.  Otherwise
+  // (host frames, several chunks, a layer an earlier call wrote) the layers are filled first and read as before.
+  bool fresh = !select_only && n <= static_cast<size_t>(kMaxFramesPerLaunch);
+  for (int k = 1; k < 4; ++k) fresh = fresh && layer_is_fresh(ctx, need[k]);
   for (int l : need) {
-    const int st = ensure_layer(ctx, l);
+    bool overwritten = false;
+    const int st = fresh && l != AMB_LAYER_ELEVATION ? ensure_layer_overwrite(ctx, l, &overwritten) : ensure_layer(ctx, l);
     if (st != AMB_OK) return st;
     if (l != AMB_LAYER_ELEVATION) wait_layer_copy(ctx, l);  // written here; elevation is only read
   }
@@ -1150,9 +1197,11 @@ int ortho_run(amb_ctx* ctx, const amb_camera* camera, const double* T_G_B, const
     a.cull_data = ctx->frame_cull.as<double>() + 12 * f0;
     a.exact_data = ctx->frame_cull.as<double>() + 12 * n + 8 * f0;
     if (select_only) {
-      launch_ortho_kernel<true>(a, tiles_i * tiles_j, s);
+      launch_ortho_kernel<true, false>(a, tiles_i * tiles_j, s);
+    } else if (fresh) {
+      launch_ortho_kernel<false, true>(a, tiles_i * tiles_j, s);
     } else {
-      launch_ortho_kernel<false>(a, tiles_i * tiles_j, s);
+      launch_ortho_kernel<false, false>(a, tiles_i * tiles_j, s);
     }
     ctx->ortho_launches += 1;
     AMB_CUDA(ctx, cudaEventRecord(guard_event, s));
