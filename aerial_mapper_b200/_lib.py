@@ -22,6 +22,7 @@ AMB_ERR_INVALID_ARGUMENT = -5
 AMB_ERR_CHECK_FAILED = -6
 AMB_ERR_NO_DEVICE = -7
 AMB_ERR_UNSUPPORTED = -8
+AMB_ERR_CORRUPT_DATA = -9
 
 LAYER_NAMES = ("ortho", "elevation", "elevation_angle", "num_observations", "elevation_angle_first_view", "delta",
                "observation_index", "observation_index_first", "colored_ortho")
@@ -157,6 +158,12 @@ SYMBOLS = {
                                          C.c_int32, _P, C.c_size_t, C.POINTER(C.c_size_t)]),
     "amb_export_jpeg": (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int32, _P, C.c_size_t,
                                   C.POINTER(C.c_size_t)]),
+    "amb_jpeg_info": (C.c_int, [_P, C.c_size_t, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int),
+                                C.POINTER(C.c_int), C.POINTER(C.c_int32)]),
+    "amb_jpeg_decode_device": (C.c_int, [_P, C.POINTER(_P), C.POINTER(C.c_size_t), C.c_size_t, C.c_int, C.POINTER(_P),
+                                         C.POINTER(C.c_size_t), C.POINTER(C.c_int)]),
+    "amb_ortho_process_jpeg": (C.c_int, [_P, C.POINTER(Camera), _P, C.POINTER(_P),
+                                         C.POINTER(C.c_size_t), C.c_size_t, C.c_int32]),
     "amb_deflate_max_size": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int, C.c_int32]),
     "amb_deflate_strips_device": (C.c_int, [_P, _P, C.c_int32, C.c_int32, C.c_size_t, C.c_int, C.c_int32, _P,
                                             C.c_size_t, C.POINTER(C.c_size_t), _P]),

@@ -564,6 +564,37 @@ class OrthoBackwardGrid(object):
         if not map.is_resident():
             map.download(self._layers_written())
 
+    def process_jpeg(self, T_G_Bs, jpeg_files, map):
+        """process() with the frames as JPEG files (a sequence of bytes-like objects, e.g. io.read_jpeg_files) in place
+        of decoded images: the frames that contribute are decoded on the device, pixel for pixel what cv2.imread
+        returns (amb_ortho_process_jpeg).  A corrupt scan of a contributing frame raises AmbError(AMB_ERR_CORRUPT_DATA)
+        after elevation_angle and observation_index have been written; the ortho layer is then left as it was."""
+        T = np.ascontiguousarray(T_G_Bs, dtype=np.float64).reshape(-1, 7)
+        n = T.shape[0]
+        if n == 0:
+            raise AmbError(_lib.AMB_ERR_EMPTY, "CHECK(!T_G_Bs.empty()) (ortho-backward-grid.cc:225)")
+        if n != len(jpeg_files):
+            raise AmbError(_lib.AMB_ERR_SIZE_MISMATCH,
+                           "CHECK(T_G_Bs.size() == images.size()) (ortho-backward-grid.cc:226)")
+        if map is None:
+            raise AmbError(_lib.AMB_ERR_INVALID_ARGUMENT, "CHECK(map) (ortho-backward-grid.cc:227)")
+        files = [_JpegFile(f) for f in jpeg_files]   # no copy of the files' bytes
+        colored = bool(self.settings_.colored_ortho)
+        ptrs = (C.c_void_p * n)(*[f.ptr for f in files])
+        sizes = (C.c_size_t * n)(*[f.size for f in files])
+        ctx = map.context()
+        if not map.is_resident():
+            map.upload(("elevation",) + self._layers_written())
+        check(lib().amb_ortho_set_brute_force(ctx, 1 if self.brute_force else 0), ctx)
+        check(lib().amb_ortho_set_dominance_cull(ctx, 1 if self.dominance_cull else 0), ctx)
+        st = lib().amb_ortho_process_jpeg(ctx, C.byref(self.ncameras_.camera), T.ctypes.data_as(C.c_void_p), ptrs,
+                                          sizes, n, 1 if colored else 0)
+        if st == _lib.AMB_ERR_CORRUPT_DATA and not map.is_resident():
+            map.download(self._layers_written()[:2])
+        check(st, ctx)
+        if not map.is_resident():
+            map.download(self._layers_written())
+
     def process_device(self, T_G_Bs, d_image_ptrs, row_step, map):
         """Frames already in HBM: d_image_ptrs is a sequence of device pointers (ints).  Asynchronous."""
         T = np.ascontiguousarray(T_G_Bs, dtype=np.float64).reshape(-1, 7)
@@ -797,6 +828,77 @@ def encode_jpeg(image, quality=95, sampling="420", restart_interval=0):
     return _jpeg_call(lambda buf, cap, size: lib().amb_jpeg_encode_device(ctx, C.c_void_p(image.data_ptr()), args[0],
                                                                           args[1], stride, *args[2:], buf, cap, size),
                       args, ctx)
+
+
+# ---- JPEG frames decoded on the device (amb_jpeg_info, amb_jpeg_decode_device) ---------------------------------------
+JPEG_SAMPLING_NAME = {0: "420", 1: "444", 2: "422"}
+
+
+class _JpegFile(object):
+    """A JPEG file handed to the library without copying it: `ptr` is the address of its `size` bytes, valid while this
+    object lives.  bytes are used in place (read only); bytearray, writable memoryviews and contiguous uint8 arrays
+    likewise; a read-only or strided view is copied once."""
+
+    def __init__(self, data):
+        if isinstance(data, np.ndarray):
+            if data.dtype != np.uint8:
+                raise ValueError("a JPEG file as an array must be uint8, got %s" % data.dtype)
+            self.keep = np.ascontiguousarray(data).reshape(-1)
+            self.ptr, self.size = self.keep.ctypes.data, self.keep.size
+            return
+        if isinstance(data, memoryview):
+            data = data if data.contiguous and not data.readonly else bytes(data)
+        if isinstance(data, bytes):
+            self.keep = data
+            self.ptr, self.size = C.cast(C.c_char_p(data), C.c_void_p).value, len(data)   # the bytes' own storage
+        elif isinstance(data, (bytearray, memoryview)):
+            n = data.nbytes if isinstance(data, memoryview) else len(data)
+            self.keep = (C.c_char * max(n, 1)).from_buffer(data) if n else C.create_string_buffer(1)
+            self.ptr, self.size = C.addressof(self.keep), n
+        else:
+            raise ValueError("a JPEG file must be bytes-like, got %s" % type(data).__name__)
+
+
+def _jpeg_info(f):
+    w, h, c, s, r = C.c_int32(), C.c_int32(), C.c_int(), C.c_int(), C.c_int32()
+    check(lib().amb_jpeg_info(C.c_void_p(f.ptr), f.size, C.byref(w), C.byref(h), C.byref(c), C.byref(s), C.byref(r)))
+    return {"width": w.value, "height": h.value, "components": c.value, "sampling": JPEG_SAMPLING_NAME[s.value],
+            "restart_interval": r.value}
+
+
+def jpeg_info(data):
+    """The header of a JPEG file (host only, no GPU): dict width, height, components (1 or 3), sampling ('444',
+    '422' or '420'; '444' for gray) and restart_interval.  AmbError(AMB_ERR_UNSUPPORTED) for a file outside the set the
+    device decoder takes, AmbError(AMB_ERR_INVALID_ARGUMENT) for one that is not a well-formed JPEG."""
+    return _jpeg_info(_JpegFile(data))
+
+
+def decode_jpeg(data_or_list, channels=3, device=0):
+    """JPEG file(s) decoded on a GPU: torch CUDA uint8 [H, W, 3] (B, G, R) for channels=3, [H, W] for channels=1, pixel
+    for pixel cv2.imread(path, IMREAD_COLOR / IMREAD_GRAYSCALE).  A list of files returns a list of tensors (decoded
+    together).  Raises AmbError with the status of the first file that cannot be decoded (AMB_ERR_UNSUPPORTED,
+    AMB_ERR_INVALID_ARGUMENT, AMB_ERR_CORRUPT_DATA)."""
+    import torch
+    if channels not in (1, 3):
+        raise ValueError("decode_jpeg: channels must be 1 or 3, got %r" % (channels,))
+    single = not isinstance(data_or_list, (list, tuple))
+    files = [_JpegFile(d) for d in ([data_or_list] if single else data_or_list)]
+    n = len(files)
+    if n == 0:
+        return []
+    infos = [_jpeg_info(f) for f in files]
+    dev = torch.device("cuda", int(device))
+    outs = [torch.empty((i["height"], i["width"], 3) if channels == 3 else (i["height"], i["width"]), dtype=torch.uint8,
+                        device=dev) for i in infos]
+    ctx = _jpeg_context(int(device))
+    torch.cuda.synchronize(dev)   # the outputs' allocation is ordered before the decode on the context's stream
+    ptrs = (C.c_void_p * n)(*[f.ptr for f in files])
+    sizes = (C.c_size_t * n)(*[f.size for f in files])
+    outp = (C.c_void_p * n)(*[o.data_ptr() for o in outs])
+    steps = (C.c_size_t * n)(*[i["width"] * channels for i in infos])
+    status = (C.c_int * n)()
+    check(lib().amb_jpeg_decode_device(ctx, ptrs, sizes, n, channels, outp, steps, status), ctx)
+    return outs[0] if single else outs
 
 
 # ---- Deflate strips of a GeoTIFF (amb_deflate_strips_device, amb_export_deflate_strips) -------------------------------

@@ -5,6 +5,7 @@
 #include <new>
 
 #include "amb_context.h"
+#include "jpeg_header.h"
 #include "dsm_plan.h"
 
 namespace amb {
@@ -247,6 +248,7 @@ const char* amb_status_string(int status) {
     case AMB_ERR_CHECK_FAILED: return "reference CHECK(alpha > 0.0) failed";
     case AMB_ERR_NO_DEVICE: return "no CUDA device";
     case AMB_ERR_UNSUPPORTED: return "unsupported configuration";
+    case AMB_ERR_CORRUPT_DATA: return "corrupt data";
     default: return "unknown status";
   }
 }
@@ -345,7 +347,7 @@ void amb_destroy(amb_ctx* ctx) {
     if (ctx->layers[l]) cudaFree(ctx->layers[l]);
   DeviceBuffer* bufs[] = {&ctx->points,  &ctx->point_ids, &ctx->intensities, &ctx->records, &ctx->records_tmp, &ctx->tile_offsets, &ctx->point_order, &ctx->bucket_flags,
                             &ctx->bin_starts, &ctx->block_sums, &ctx->empty_cells,
-                          &ctx->counters, &ctx->dbg_count, &ctx->dbg_level,  &ctx->raster_band, &ctx->raster_taps, &ctx->jpeg_mcu, &ctx->jpeg_spine, &ctx->jpeg_words, &ctx->jpeg_out, &ctx->deflate_scratch, &ctx->deflate_words, &ctx->cog_levels, &ctx->cog_tiles, &ctx->frames,     &ctx->frame_table,
+                          &ctx->counters, &ctx->dbg_count, &ctx->dbg_level,  &ctx->raster_band, &ctx->raster_taps, &ctx->jpeg_mcu, &ctx->jpeg_spine, &ctx->jpeg_words, &ctx->jpeg_out, &ctx->jdec_files, &ctx->jdec_stream, &ctx->jdec_meta, &ctx->jdec_subs, &ctx->jdec_coef, &ctx->deflate_scratch, &ctx->deflate_words, &ctx->cog_levels, &ctx->cog_tiles, &ctx->frames,     &ctx->frame_table,
                           &ctx->frame_cull, &ctx->frame_rects, &ctx->ortho_pix, &ctx->ortho_bbox};
   for (DeviceBuffer* b : bufs) b->release();
   for (int k = 0; k < EV_COUNT; ++k)
@@ -692,6 +694,36 @@ int amb_ortho_process(amb_ctx* ctx, const amb_camera* camera, const double* T_G_
   ctx->ortho_had_h2d = true;
   ctx->ortho_two_phase = true;
   int st = ortho_run(ctx, camera, T_G_B, nullptr, images, n, channels, row_step, colored_ortho);
+  if (st != AMB_OK) return st;
+  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_ORTHO_END], ctx->stream));
+  ctx->ortho_timed = true;
+  return finish_flags(ctx, CTR_ORTHO_CHECK, AMB_ERR_CHECK_FAILED);
+}
+
+int amb_ortho_process_jpeg(amb_ctx* ctx, const amb_camera* camera, const double* T_G_B, const void* const* files,
+                           const size_t* file_bytes, size_t n, int32_t colored_ortho) {
+  if (!ctx) return AMB_ERR_INVALID_ARGUMENT;
+  if (n == 0) return AMB_ERR_EMPTY;
+  if (!camera || !T_G_B || !files || !file_bytes) return AMB_ERR_INVALID_ARGUMENT;
+  if (camera->width <= 0 || camera->height <= 0) return AMB_ERR_SIZE_MISMATCH;
+  // every header before any device work: nothing is touched if one frame cannot be decoded
+  std::vector<JpegFrame> headers(n);
+  for (size_t f = 0; f < n; ++f) {
+    if (!files[f]) return AMB_ERR_INVALID_ARGUMENT;
+    const int st = jpeg_parse(static_cast<const unsigned char*>(files[f]), file_bytes[f], &headers[f]);
+    if (st != AMB_OK) return st;
+  }
+  for (size_t f = 0; f < n; ++f)
+    if (headers[f].width != camera->width || headers[f].height != camera->height) return AMB_ERR_SIZE_MISMATCH;
+  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
+  const int32_t channels = colored_ortho ? 3 : 1;
+  JpegBands jpeg{files, file_bytes, headers.data(), nullptr, nullptr, n, channels};
+  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_ORTHO_BEGIN], ctx->stream));
+  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_ORTHO_H2D_END], ctx->stream));
+  ctx->ortho_had_h2d = true;
+  ctx->ortho_two_phase = true;
+  int st = ortho_run(ctx, camera, T_G_B, nullptr, nullptr, n, channels,
+                     static_cast<size_t>(camera->width) * channels, colored_ortho, &jpeg);
   if (st != AMB_OK) return st;
   AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_ORTHO_END], ctx->stream));
   ctx->ortho_timed = true;

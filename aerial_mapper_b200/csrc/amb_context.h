@@ -190,6 +190,11 @@ struct amb_ctx {
   amb::DeviceBuffer jpeg_spine;   // ... tile sums of its scans
   amb::DeviceBuffer jpeg_words;   // ... the entropy-coded stream before byte stuffing, and 0xFF counts per chunk
   amb::DeviceBuffer jpeg_out;     // ... the stuffed stream with its RST markers, copied to the host
+  amb::DeviceBuffer jdec_files;   // JPEG decoder (jpeg_decode.cu): the files of a group
+  amb::DeviceBuffer jdec_stream;  // ... their scans without byte stuffing and restart markers
+  amb::DeviceBuffer jdec_meta;    // ... per-frame tables, chunk table and its scan, restart-segment starts, status flags
+  amb::DeviceBuffer jdec_subs;    // ... subsequences, their entry states and the scans of their block / DC counts
+  amb::DeviceBuffer jdec_coef;    // ... coefficients (MCU order), then the 8-bit component planes
   amb::DeviceBuffer deflate_scratch;  // Deflate encoder (deflate_encode.cu): predicted bytes, tokens, per-segment,
                                      // per-block and per-strip tables
   amb::DeviceBuffer deflate_words;    // ... the zlib streams of all strips, copied to the host
@@ -291,8 +296,12 @@ int dsm_extract_halo(amb_ctx* ctx, const double* d_xyz, const unsigned long long
 int pcl_adaptive_prepare(amb_ctx* ctx, float** saved);
 int pcl_adaptive_finish(amb_ctx* ctx, int pass_status, const double* d_xyz, const unsigned long long* d_ids,
                         const int* d_intensities, size_t n, int32_t interpolation_radius, float* saved);
+struct JpegBands;  // jpeg_header.h
+// jpeg (host-frame path only, h_images == nullptr): the frames are JPEG files; the rows of each frame's bounding box of
+// winner pixels are decoded on the device in place of the rectangle copies (jpeg->row0 / row1 are filled here)
 int ortho_run(amb_ctx* ctx, const amb_camera* camera, const double* T_G_B, const uint8_t* const* d_images,
-              const uint8_t* const* h_images, size_t n, int32_t channels, size_t row_step, int32_t colored_ortho);
+              const uint8_t* const* h_images, size_t n, int32_t channels, size_t row_step, int32_t colored_ortho,
+              JpegBands* jpeg = nullptr);
 // amb_comm.cu: one step of a sharded cloud on a context of a communicator of several ranks (halo exchange, then
 // dsm_run over the rank's points and the neighbours' halos); records the DSM events and sets dsm_timed itself
 int sharded_step(amb_ctx* ctx, const double* d_xyz, const int* d_intensities, const uint64_t* d_ids, size_t n_local,

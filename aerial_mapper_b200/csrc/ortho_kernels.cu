@@ -19,6 +19,7 @@
 #include <mutex>
 
 #include "amb_context.h"
+#include "jpeg_header.h"
 #include "approx_math.h"
 
 namespace amb {
@@ -979,9 +980,9 @@ double distortion_slope(const amb_camera& cam, double r) {
 //   is seen by ~8 frames but takes its pixel from one.
 int ortho_run(amb_ctx* ctx, const amb_camera* camera, const double* T_G_B, const uint8_t* const* d_images,
               const uint8_t* const* h_images, size_t n, int32_t channels, size_t row_step,
-              int32_t colored_ortho) {
+              int32_t colored_ortho, JpegBands* jpeg) {
   if (n == 0) return AMB_ERR_EMPTY;  // CHECK(!T_G_Bs.empty()), ortho-backward-grid.cc:225
-  if (!camera || !T_G_B || (!d_images && !h_images)) return AMB_ERR_INVALID_ARGUMENT;
+  if (!camera || !T_G_B || (!d_images && !h_images && !jpeg)) return AMB_ERR_INVALID_ARGUMENT;
   const bool select_only = d_images == nullptr;
   if (camera->width > 65535 || camera->height > 65535) return AMB_ERR_UNSUPPORTED;
   if (colored_ortho ? channels != 3 : channels != 1) return AMB_ERR_SIZE_MISMATCH;
@@ -1227,41 +1228,65 @@ int ortho_run(amb_ctx* ctx, const amb_camera* camera, const double* T_G_B, const
   AMB_CUDA(ctx, cudaStreamSynchronize(s));
   bbox = bbox_back;
   FrameRect* rects = stage.take<FrameRect>(n);
-  size_t total = 0;
-  for (size_t f = 0; f < n; ++f) {
-    FrameRect& r = rects[f];
-    r.ptr = nullptr;
-    r.x0 = r.y0 = r.pitch = r.pad_ = 0;
-    if (bbox[4 * f + 2] < 0) continue;  // no cell takes its pixel from this frame
-    const int w = bbox[4 * f + 2] - bbox[4 * f + 0] + 1;
-    r.x0 = bbox[4 * f + 0];
-    r.y0 = bbox[4 * f + 1];
-    r.pitch = static_cast<int>((static_cast<size_t>(w) * channels + 255) & ~static_cast<size_t>(255));
-    r.pad_ = bbox[4 * f + 3] - bbox[4 * f + 1] + 1;  // rows
-    total += static_cast<size_t>(r.pitch) * r.pad_;
-  }
-  AMB_CUDA(ctx, ctx->frames.reserve(total + 256));
   AMB_CUDA(ctx, ctx->frame_rects.reserve(n * sizeof(FrameRect)));
-  size_t off = 0;
-  std::vector<StagedRect> copies;
-  copies.reserve(n);
-  for (size_t f = 0; f < n; ++f) {
-    FrameRect& r = rects[f];
-    if (bbox[4 * f + 2] < 0) continue;
-    const int w = bbox[4 * f + 2] - r.x0 + 1, h = r.pad_;
-    uint8_t* dst = ctx->frames.as<uint8_t>() + off;
-    const uint8_t* src = h_images[f] + static_cast<size_t>(r.y0) * row_step + static_cast<size_t>(r.x0) * channels;
-    // (frames in pageable memory — cv::Mat storage — are packed into pinned slots by the worker pool: host_staging.cu)
-    copies.push_back(StagedRect{dst, static_cast<size_t>(r.pitch), src, row_step, static_cast<size_t>(w) * channels,
-                                static_cast<size_t>(h)});
-    ctx->ortho_h2d_bytes += static_cast<int64_t>(w) * channels * h;
-    r.ptr = dst;
-    off += static_cast<size_t>(r.pitch) * h;
-    r.pad_ = 0;
-  }
-  {
-    const int cst = staged_h2d_rects(ctx, copies.data(), copies.size(), s);
-    if (cst != AMB_OK) return cst;
+  if (jpeg) {
+    // JPEG frames: the rows of each frame's box, every column, decoded on the device (frames without a winner are
+    // neither copied nor decoded)
+    std::vector<int32_t> row0(n), row1(n);
+    std::vector<unsigned char*> ptr(n);
+    std::vector<int> pitch(n);
+    for (size_t f = 0; f < n; ++f) {
+      row0[f] = bbox[4 * f + 2] < 0 ? 0 : bbox[4 * f + 1];
+      row1[f] = bbox[4 * f + 2] < 0 ? 0 : bbox[4 * f + 3] + 1;
+    }
+    jpeg->row0 = row0.data();
+    jpeg->row1 = row1.data();
+    const int dst = jpeg_decode_bands(ctx, *jpeg, ptr.data(), pitch.data());
+    if (dst != AMB_OK) return dst;
+    for (size_t f = 0; f < n; ++f) {
+      rects[f].ptr = ptr[f];
+      rects[f].x0 = 0;
+      rects[f].y0 = row0[f];
+      rects[f].pitch = pitch[f];
+      rects[f].pad_ = 0;
+      if (ptr[f]) ctx->ortho_h2d_bytes += static_cast<int64_t>(jpeg->file_bytes[f]);
+    }
+  } else {
+    size_t total = 0;
+    for (size_t f = 0; f < n; ++f) {
+      FrameRect& r = rects[f];
+      r.ptr = nullptr;
+      r.x0 = r.y0 = r.pitch = r.pad_ = 0;
+      if (bbox[4 * f + 2] < 0) continue;  // no cell takes its pixel from this frame
+      const int w = bbox[4 * f + 2] - bbox[4 * f + 0] + 1;
+      r.x0 = bbox[4 * f + 0];
+      r.y0 = bbox[4 * f + 1];
+      r.pitch = static_cast<int>((static_cast<size_t>(w) * channels + 255) & ~static_cast<size_t>(255));
+      r.pad_ = bbox[4 * f + 3] - bbox[4 * f + 1] + 1;  // rows
+      total += static_cast<size_t>(r.pitch) * r.pad_;
+    }
+    AMB_CUDA(ctx, ctx->frames.reserve(total + 256));
+    size_t off = 0;
+    std::vector<StagedRect> copies;
+    copies.reserve(n);
+    for (size_t f = 0; f < n; ++f) {
+      FrameRect& r = rects[f];
+      if (bbox[4 * f + 2] < 0) continue;
+      const int w = bbox[4 * f + 2] - r.x0 + 1, h = r.pad_;
+      uint8_t* dst = ctx->frames.as<uint8_t>() + off;
+      const uint8_t* src = h_images[f] + static_cast<size_t>(r.y0) * row_step + static_cast<size_t>(r.x0) * channels;
+      // (frames in pageable memory — cv::Mat storage — are packed into pinned slots by the worker pool: host_staging.cu)
+      copies.push_back(StagedRect{dst, static_cast<size_t>(r.pitch), src, row_step, static_cast<size_t>(w) * channels,
+                                  static_cast<size_t>(h)});
+      ctx->ortho_h2d_bytes += static_cast<int64_t>(w) * channels * h;
+      r.ptr = dst;
+      off += static_cast<size_t>(r.pitch) * h;
+      r.pad_ = 0;
+    }
+    {
+      const int cst = staged_h2d_rects(ctx, copies.data(), copies.size(), s);
+      if (cst != AMB_OK) return cst;
+    }
   }
   AMB_CUDA(ctx, cudaMemcpyAsync(ctx->frame_rects.ptr, rects, n * sizeof(FrameRect), cudaMemcpyHostToDevice, s));
   AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_ORTHO_COPY_END], s));

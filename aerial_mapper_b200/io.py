@@ -4,6 +4,7 @@
     load_poses_from_file_standard   :103-121   text stream  x y z qw qx qy qz
     load_point_cloud_from_file      :309-347   text stream  x y z intensity, keeps z > -100
     load_images_from_file           :207-227   <prefix><i>.jpg, gray (IMREAD_GRAYSCALE) or colour (BGR)
+    read_jpeg_files                            the same files undecoded, for OrthoBackwardGrid.process_jpeg
     load_camera_rig_from_file       :251-261   aslam NCamera YAML (camera 0: pinhole + distortion, T_B_C)
 
 and the output side ("next" row N4):
@@ -91,6 +92,22 @@ def load_images_from_file(filename_base, num_poses, load_colored_images=False):
     if not images:
         raise ValueError("No images loaded.")
     return images
+
+
+def read_jpeg_files(filename_base, num_poses):
+    """The raw bytes of filename_base + str(i) + ".jpg" for i in [0, num_poses), the names load_images_from_file reads,
+    with its errors: for OrthoBackwardGrid.process_jpeg, which decodes the frames that contribute on the device."""
+    files = []
+    for i in range(int(num_poses)):
+        name = "%s%d.jpg" % (filename_base, i)
+        try:
+            with open(name, "rb") as f:
+                files.append(f.read())
+        except OSError:
+            raise IOError("cannot read %s" % name)
+    if not files:
+        raise ValueError("No images loaded.")
+    return files
 
 
 def _matrix(node):

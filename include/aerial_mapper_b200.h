@@ -43,7 +43,8 @@ typedef enum amb_status {
   AMB_ERR_INVALID_ARGUMENT = -5,
   AMB_ERR_CHECK_FAILED = -6,     /* reference CHECK(alpha > 0.0), ortho-backward-grid.cc:178 */
   AMB_ERR_NO_DEVICE = -7,
-  AMB_ERR_UNSUPPORTED = -8
+  AMB_ERR_UNSUPPORTED = -8,
+  AMB_ERR_CORRUPT_DATA = -9      /* a JPEG scan that is not valid for its header (amb_jpeg_decode_device) */
 } amb_status;
 
 /* Geometry of the grid_map (grid_map::GridMap::setGeometry as called at aerial-mapper-grid-map.cc:30-33). */
@@ -509,7 +510,7 @@ int amb_raster_import_tables(const amb_geometry* geom, int32_t col_begin, int32_
  * Errors: a NULL pointer, width or height <= 0, or a short row_stride returns AMB_ERR_INVALID_ARGUMENT; a parameter
  * outside the supported set (a side over 65535, channels, quality, sampling, restart interval) AMB_ERR_UNSUPPORTED.
  * Neither writes anything. */
-typedef enum amb_jpeg_sampling { AMB_JPEG_420 = 0, AMB_JPEG_444 = 1 } amb_jpeg_sampling;
+typedef enum amb_jpeg_sampling { AMB_JPEG_420 = 0, AMB_JPEG_444 = 1, AMB_JPEG_422 = 2 /* decoder only */ } amb_jpeg_sampling;
 /* Host arithmetic, no GPU: an upper bound on the file size (markers and byte stuffing included); 0 if unsupported. */
 size_t amb_jpeg_max_size(int32_t width, int32_t height, int channels, int quality, int sampling,
                          int32_t restart_interval);
@@ -523,6 +524,51 @@ int amb_jpeg_encode_device(amb_ctx* ctx, const void* d_image, int32_t width, int
  * amb_jpeg_encode_device of it: the context's band (image rows [col_begin, col_end)) as an image of its own. */
 int amb_export_jpeg(amb_ctx* ctx, int layer, int format, int quality, int sampling, int32_t restart_interval,
                     void* host_out, size_t capacity, size_t* size);
+
+/* ---- JPEG frames decoded on the device ----
+ * Convention.  The output is byte for byte cv2.imread(path, IMREAD_COLOR) (channels 3: B, G, R bytes) or
+ * cv2.imread(path, IMREAD_GRAYSCALE) (channels 1) of the same file, OpenCV 4.13 with libjpeg-turbo 3.1.2 at its default
+ * decompression settings: islow integer IDCT (jidctint.c, with its `& RANGE_MASK` range limit), the DC predictor an
+ * int stored as a 16-bit coefficient, fancy upsampling (jdsample.c h2v1 / h2v2 triangle filters; edges replicate the
+ * last real chroma row or column; box replication when the chroma plane is at most 2 samples wide) and jdcolor.c's
+ * table-based YCbCr -> BGR.  Gray output of a colour file is its Y plane; colour output of a gray file repeats the gray
+ * value.
+ * Supported: sequential baseline (SOF0) and extended sequential Huffman (SOF1) with 8-bit samples and one scan holding
+ * every component; 1 component (gray) or 3 (YCbCr, JFIF) at 4:4:4, 4:2:2 (h2v1) or 4:2:0 (h2v2): luma factors 1x1,
+ * 2x1 or 2x2, chroma 1x1; any DQT (8- or 16-bit) and DHT; any restart interval.  APPn and COM segments are skipped;
+ * anything after the last MCU is ignored.  Refused with AMB_ERR_UNSUPPORTED, before anything is written: progressive,
+ * arithmetic coding, 12/16-bit samples, lossless, hierarchical, multi-scan sequential, 2 or 4 components, an Adobe
+ * segment (colour transforms, CMYK / YCCK), three components named R, G, B without JFIF, other sampling factors, DNL,
+ * an EXIF orientation other than 1 (cv2.imread would rotate the image), Huffman tables the stream leaves out.  A stream
+ * that is not JPEG or whose header is malformed returns AMB_ERR_INVALID_ARGUMENT.
+ * Difference from cv2: a scan that is not valid for its header (a code no table holds, a run past coefficient 63, an
+ * RSTn out of sequence or missing, an RSTn past those the restart interval calls for before the last MCU, data ending
+ * before the last MCU) returns AMB_ERR_CORRUPT_DATA, where libjpeg-turbo warns and substitutes zeros. */
+/* Host only, no GPU: parses and checks the header; sampling is an amb_jpeg_sampling (AMB_JPEG_444 for gray).  Any
+ * output pointer may be NULL. */
+int amb_jpeg_info(const void* file, size_t bytes, int32_t* width, int32_t* height, int* components, int* sampling,
+                  int32_t* restart_interval);
+/* Decodes n files in host memory (pinned or pageable) into device rasters d_out[i] (height rows of width * channels
+ * bytes, row_step[i] bytes apart) on the context's stream, after earlier work on it.  Synchronous: corruption is found
+ * on the device.  status[i] is that frame's result (AMB_OK, AMB_ERR_UNSUPPORTED, AMB_ERR_INVALID_ARGUMENT for a bad
+ * header, a NULL destination or a short row_step, AMB_ERR_CORRUPT_DATA); a frame that fails is left unwritten and the
+ * others are decoded.  Returns the first frame's non-OK status, or AMB_OK; AMB_ERR_INVALID_ARGUMENT for a NULL array or
+ * channels other than 1 or 3.  The frames go through the kernels in groups whose device scratch stays under 1 GiB (a
+ * frame that alone needs more forms a group of its own): the file and its unstuffed scan, 192 bytes per 8x8 block
+ * (coefficients and planes) and 80 bytes per KB of scan. */
+int amb_jpeg_decode_device(amb_ctx* ctx, const void* const* files, const size_t* file_bytes, size_t n, int channels,
+                           void* const* d_out, const size_t* row_step, int* status);
+
+/* amb_ortho_process with JPEG files (host memory, pinned or pageable) in place of decoded frames, the frames decoded on
+ * the device as amb_jpeg_decode_device would (colored_ortho: BGR, else gray).  Every header is parsed first: a frame
+ * whose size differs from the camera's returns AMB_ERR_SIZE_MISMATCH, one outside the supported set AMB_ERR_UNSUPPORTED
+ * (a malformed one AMB_ERR_INVALID_ARGUMENT), and no layer is touched.  Then the winners are selected as
+ * amb_ortho_process does, and only the frames that contribute are copied to the device and decoded, only the rows of
+ * their bounding box of winner pixels (plus the MCU rows around them the upsampling needs).  A contributing frame whose
+ * scan is corrupt returns AMB_ERR_CORRUPT_DATA: elevation_angle and observation_index then hold the selection and the
+ * ortho layer is not written.  A frame that contributes nothing is never decoded, so its scan is not checked. */
+int amb_ortho_process_jpeg(amb_ctx* ctx, const amb_camera* camera, const double* T_G_B, const void* const* files,
+                           const size_t* file_bytes, size_t n, int32_t colored_ortho);
 
 /* ---- Deflate-compressed GeoTIFF strips ----
  * Convention.  The strips of a classic TIFF with Compression = 8 (Adobe Deflate), PlanarConfiguration 1 and
