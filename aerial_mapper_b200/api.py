@@ -530,15 +530,26 @@ class OrthoBackwardGrid(object):
         out = "colored_ortho" if self.settings_.colored_ortho else "ortho"
         return ("elevation_angle", "observation_index", out)
 
-    def process(self, T_G_Bs, images, map):
-        """T_G_Bs: float64 [n, 7] rows x y z qw qx qy qz; images: n uint8 arrays [H, W] (gray) or [H, W, 3] (BGR)."""
+    def _configure(self, ctx):
+        """This grid's brute_force and dominance_cull onto the map's context, before each of its calls."""
+        check(lib().amb_ortho_set_brute_force(ctx, 1 if self.brute_force else 0), ctx)
+        check(lib().amb_ortho_set_dominance_cull(ctx, 1 if self.dominance_cull else 0), ctx)
+
+    @staticmethod
+    def _poses(T_G_Bs, frames, empty=_lib.AMB_ERR_EMPTY):
+        """T_G_Bs as float64 [n, 7] and n, one frame per pose (ortho-backward-grid.cc:225-226)."""
         T = np.ascontiguousarray(T_G_Bs, dtype=np.float64).reshape(-1, 7)
         n = T.shape[0]
         if n == 0:
-            raise AmbError(_lib.AMB_ERR_EMPTY, "CHECK(!T_G_Bs.empty()) (ortho-backward-grid.cc:225)")
-        if n != len(images):
+            raise AmbError(empty, "CHECK(!T_G_Bs.empty()) (ortho-backward-grid.cc:225)")
+        if n != len(frames):
             raise AmbError(_lib.AMB_ERR_SIZE_MISMATCH,
                            "CHECK(T_G_Bs.size() == images.size()) (ortho-backward-grid.cc:226)")
+        return T, n
+
+    def process(self, T_G_Bs, images, map):
+        """T_G_Bs: float64 [n, 7] rows x y z qw qx qy qz; images: n uint8 arrays [H, W] (gray) or [H, W, 3] (BGR)."""
+        T, n = self._poses(T_G_Bs, images)
         if map is None:
             raise AmbError(_lib.AMB_ERR_INVALID_ARGUMENT, "CHECK(map) (ortho-backward-grid.cc:227)")
         colored = bool(self.settings_.colored_ortho)
@@ -557,8 +568,7 @@ class OrthoBackwardGrid(object):
         ctx = map.context()
         if not map.is_resident():
             map.upload(("elevation",) + self._layers_written())
-        check(lib().amb_ortho_set_brute_force(ctx, 1 if self.brute_force else 0), ctx)
-        check(lib().amb_ortho_set_dominance_cull(ctx, 1 if self.dominance_cull else 0), ctx)
+        self._configure(ctx)
         check(lib().amb_ortho_process(ctx, C.byref(cam), T.ctypes.data_as(C.c_void_p), C.cast(ptrs, C.c_void_p), n,
                                       channels, row_step, 1 if colored else 0), ctx)
         if not map.is_resident():
@@ -569,13 +579,7 @@ class OrthoBackwardGrid(object):
         of decoded images: the frames that contribute are decoded on the device, pixel for pixel what cv2.imread
         returns (amb_ortho_process_jpeg).  A corrupt scan of a contributing frame raises AmbError(AMB_ERR_CORRUPT_DATA)
         after elevation_angle and observation_index have been written; the ortho layer is then left as it was."""
-        T = np.ascontiguousarray(T_G_Bs, dtype=np.float64).reshape(-1, 7)
-        n = T.shape[0]
-        if n == 0:
-            raise AmbError(_lib.AMB_ERR_EMPTY, "CHECK(!T_G_Bs.empty()) (ortho-backward-grid.cc:225)")
-        if n != len(jpeg_files):
-            raise AmbError(_lib.AMB_ERR_SIZE_MISMATCH,
-                           "CHECK(T_G_Bs.size() == images.size()) (ortho-backward-grid.cc:226)")
+        T, n = self._poses(T_G_Bs, jpeg_files)
         if map is None:
             raise AmbError(_lib.AMB_ERR_INVALID_ARGUMENT, "CHECK(map) (ortho-backward-grid.cc:227)")
         files = [_JpegFile(f) for f in jpeg_files]   # no copy of the files' bytes
@@ -585,8 +589,7 @@ class OrthoBackwardGrid(object):
         ctx = map.context()
         if not map.is_resident():
             map.upload(("elevation",) + self._layers_written())
-        check(lib().amb_ortho_set_brute_force(ctx, 1 if self.brute_force else 0), ctx)
-        check(lib().amb_ortho_set_dominance_cull(ctx, 1 if self.dominance_cull else 0), ctx)
+        self._configure(ctx)
         st = lib().amb_ortho_process_jpeg(ctx, C.byref(self.ncameras_.camera), T.ctypes.data_as(C.c_void_p), ptrs,
                                           sizes, n, 1 if colored else 0)
         if st == _lib.AMB_ERR_CORRUPT_DATA and not map.is_resident():
@@ -597,15 +600,11 @@ class OrthoBackwardGrid(object):
 
     def process_device(self, T_G_Bs, d_image_ptrs, row_step, map):
         """Frames already in HBM: d_image_ptrs is a sequence of device pointers (ints).  Asynchronous."""
-        T = np.ascontiguousarray(T_G_Bs, dtype=np.float64).reshape(-1, 7)
-        n = T.shape[0]
-        if n == 0 or n != len(d_image_ptrs):
-            raise AmbError(_lib.AMB_ERR_SIZE_MISMATCH)
+        T, n = self._poses(T_G_Bs, d_image_ptrs, empty=_lib.AMB_ERR_SIZE_MISMATCH)
         colored = bool(self.settings_.colored_ortho)
         ptrs = (C.c_void_p * n)(*[int(p) for p in d_image_ptrs])
         ctx = map.context()
-        check(lib().amb_ortho_set_brute_force(ctx, 1 if self.brute_force else 0), ctx)
-        check(lib().amb_ortho_set_dominance_cull(ctx, 1 if self.dominance_cull else 0), ctx)
+        self._configure(ctx)
         check(lib().amb_ortho_process_device(ctx, C.byref(self.ncameras_.camera), T.ctypes.data_as(C.c_void_p),
                                              C.cast(ptrs, C.c_void_p), n, 3 if colored else 1, int(row_step),
                                              1 if colored else 0), ctx)

@@ -229,6 +229,44 @@ static int run_cloud(amb_ctx* ctx, const CloudCall& c) {
   return AMB_OK;
 }
 
+// One OrthoBackwardGrid::process, wherever its frames live: every amb_ortho_process* entry point is one call of
+// run_ortho.  Every argument is checked before any device work, so a refused call leaves the layers and the previous
+// call's timings as they were.
+static int run_ortho(amb_ctx* ctx, OrthoCall c) {
+  if (!ctx) return AMB_ERR_INVALID_ARGUMENT;
+  if (c.n == 0) return AMB_ERR_EMPTY;  // CHECK(!T_G_Bs.empty()), ortho-backward-grid.cc:225
+  const bool jpeg = c.frames == OrthoCall::JPEG;
+  if (!c.camera || !c.T_G_B || (jpeg ? !c.files || !c.file_bytes : !c.images)) return AMB_ERR_INVALID_ARGUMENT;
+  const amb_camera& cam = *c.camera;
+  if (cam.width <= 0 || cam.height <= 0) return AMB_ERR_SIZE_MISMATCH;
+  std::vector<JpegFrame> headers(jpeg ? c.n : 0);  // every header before any device work
+  for (size_t f = 0; f < c.n && c.frames != OrthoCall::DEVICE; ++f) {  // device frame pointers are not inspected
+    if (jpeg ? !c.files[f] : !c.images[f]) return AMB_ERR_INVALID_ARGUMENT;
+    if (!jpeg) continue;
+    const int st = jpeg_parse(static_cast<const unsigned char*>(c.files[f]), c.file_bytes[f], &headers[f]);
+    if (st != AMB_OK) return st;
+  }
+  for (const JpegFrame& h : headers)
+    if (h.width != cam.width || h.height != cam.height) return AMB_ERR_SIZE_MISMATCH;
+  c.headers = headers.data();
+  if (jpeg) c.row_step = static_cast<size_t>(cam.width) * c.channels;  // decoded bands: rows of width * channels
+  if (cam.width > 65535 || cam.height > 65535) return AMB_ERR_UNSUPPORTED;
+  if (c.colored_ortho ? c.channels != 3 : c.channels != 1) return AMB_ERR_SIZE_MISMATCH;
+  if (c.row_step < static_cast<size_t>(cam.width) * c.channels) return AMB_ERR_SIZE_MISMATCH;
+  if (cam.dist_type < AMB_DIST_NONE || cam.dist_type > AMB_DIST_FOV) return AMB_ERR_UNSUPPORTED;
+  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
+  ctx->ortho_timed = false;  // the events below are this call's: its timings stand only if it succeeds
+  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_ORTHO_BEGIN], ctx->stream));
+  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_ORTHO_H2D_END], ctx->stream));
+  ctx->ortho_two_phase = c.frames != OrthoCall::DEVICE;
+  const int st = ortho_run(ctx, c);
+  if (st != AMB_OK) return st;
+  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_ORTHO_END], ctx->stream));
+  ctx->ortho_timed = true;
+  // host and JPEG frames return with their result final and CHECK(alpha > 0) reported; device frames leave it to amb_sync
+  return c.frames == OrthoCall::DEVICE ? AMB_OK : finish_flags(ctx, CTR_ORTHO_CHECK, AMB_ERR_CHECK_FAILED);
+}
+
 }  // namespace amb
 
 using namespace amb;
@@ -668,66 +706,21 @@ int amb_dsm_thresholds(int32_t interpolation_radius, double* thresholds, int32_t
 int amb_ortho_process_device(amb_ctx* ctx, const amb_camera* camera, const double* T_G_B,
                              const uint8_t* const* d_images, size_t n, int32_t channels, size_t row_step,
                              int32_t colored_ortho) {
-  if (!ctx) return AMB_ERR_INVALID_ARGUMENT;
-  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
-  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_ORTHO_BEGIN], ctx->stream));
-  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_ORTHO_H2D_END], ctx->stream));
-  ctx->ortho_had_h2d = false;
-  ctx->ortho_two_phase = false;
-  int st = ortho_run(ctx, camera, T_G_B, d_images, nullptr, n, channels, row_step, colored_ortho);
-  if (st == AMB_OK) AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_ORTHO_END], ctx->stream));
-  ctx->ortho_timed = (st == AMB_OK);
-  return st;
+  return run_ortho(ctx, {.frames = OrthoCall::DEVICE, .camera = camera, .T_G_B = T_G_B, .n = n, .channels = channels,
+                         .row_step = row_step, .colored_ortho = colored_ortho, .images = d_images});
 }
 
 int amb_ortho_process(amb_ctx* ctx, const amb_camera* camera, const double* T_G_B, const uint8_t* const* images,
                       size_t n, int32_t channels, size_t row_step, int32_t colored_ortho) {
-  if (!ctx) return AMB_ERR_INVALID_ARGUMENT;
-  if (n == 0) return AMB_ERR_EMPTY;
-  if (!camera || !T_G_B || !images) return AMB_ERR_INVALID_ARGUMENT;
-  if (camera->width <= 0 || camera->height <= 0) return AMB_ERR_SIZE_MISMATCH;
-  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
-  for (size_t f = 0; f < n; ++f)
-    if (!images[f]) return AMB_ERR_INVALID_ARGUMENT;
-  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_ORTHO_BEGIN], ctx->stream));
-  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_ORTHO_H2D_END], ctx->stream));
-  ctx->ortho_had_h2d = true;
-  ctx->ortho_two_phase = true;
-  int st = ortho_run(ctx, camera, T_G_B, nullptr, images, n, channels, row_step, colored_ortho);
-  if (st != AMB_OK) return st;
-  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_ORTHO_END], ctx->stream));
-  ctx->ortho_timed = true;
-  return finish_flags(ctx, CTR_ORTHO_CHECK, AMB_ERR_CHECK_FAILED);
+  return run_ortho(ctx, {.frames = OrthoCall::HOST, .camera = camera, .T_G_B = T_G_B, .n = n, .channels = channels,
+                         .row_step = row_step, .colored_ortho = colored_ortho, .images = images});
 }
 
 int amb_ortho_process_jpeg(amb_ctx* ctx, const amb_camera* camera, const double* T_G_B, const void* const* files,
                            const size_t* file_bytes, size_t n, int32_t colored_ortho) {
-  if (!ctx) return AMB_ERR_INVALID_ARGUMENT;
-  if (n == 0) return AMB_ERR_EMPTY;
-  if (!camera || !T_G_B || !files || !file_bytes) return AMB_ERR_INVALID_ARGUMENT;
-  if (camera->width <= 0 || camera->height <= 0) return AMB_ERR_SIZE_MISMATCH;
-  // every header before any device work: nothing is touched if one frame cannot be decoded
-  std::vector<JpegFrame> headers(n);
-  for (size_t f = 0; f < n; ++f) {
-    if (!files[f]) return AMB_ERR_INVALID_ARGUMENT;
-    const int st = jpeg_parse(static_cast<const unsigned char*>(files[f]), file_bytes[f], &headers[f]);
-    if (st != AMB_OK) return st;
-  }
-  for (size_t f = 0; f < n; ++f)
-    if (headers[f].width != camera->width || headers[f].height != camera->height) return AMB_ERR_SIZE_MISMATCH;
-  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
-  const int32_t channels = colored_ortho ? 3 : 1;
-  JpegBands jpeg{files, file_bytes, headers.data(), nullptr, nullptr, n, channels};
-  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_ORTHO_BEGIN], ctx->stream));
-  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_ORTHO_H2D_END], ctx->stream));
-  ctx->ortho_had_h2d = true;
-  ctx->ortho_two_phase = true;
-  int st = ortho_run(ctx, camera, T_G_B, nullptr, nullptr, n, channels,
-                     static_cast<size_t>(camera->width) * channels, colored_ortho, &jpeg);
-  if (st != AMB_OK) return st;
-  AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_ORTHO_END], ctx->stream));
-  ctx->ortho_timed = true;
-  return finish_flags(ctx, CTR_ORTHO_CHECK, AMB_ERR_CHECK_FAILED);
+  return run_ortho(ctx, {.frames = OrthoCall::JPEG, .camera = camera, .T_G_B = T_G_B, .n = n,
+                         .channels = colored_ortho ? 3 : 1, .colored_ortho = colored_ortho, .files = files,
+                         .file_bytes = file_bytes});
 }
 
 int amb_ortho_set_brute_force(amb_ctx* ctx, int brute_force) {

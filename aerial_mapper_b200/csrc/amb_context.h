@@ -157,7 +157,7 @@ struct amb_ctx {
   amb::CompactMirror compact[AMB_NUM_LAYERS];  // opt-in one-byte transport (amb_set_host_mirror_compact)
   cudaEvent_t layer_copy_event[AMB_NUM_LAYERS] = {};  // completion of an asynchronous download of that layer
   bool layer_copy_pending[AMB_NUM_LAYERS] = {};
-  bool dsm_timed = false, ortho_timed = false, dsm_had_h2d = false, ortho_had_h2d = false;
+  bool dsm_timed = false, ortho_timed = false, dsm_had_h2d = false;
   int32_t dsm_launches = 0, ortho_launches = 0;
   std::string last_error;
 
@@ -228,7 +228,7 @@ struct amb_ctx {
   amb::DeviceBuffer ortho_pix;    // host-frame path: winner pixel per cell
   amb::DeviceBuffer ortho_bbox;   // host-frame path: per-frame bounding box of the winners' pixels
   int64_t ortho_h2d_bytes = 0;
-  bool ortho_two_phase = false;
+  bool ortho_two_phase = false;   // the last ortho call had host or JPEG frames: select kernel | copies | texel kernel
   bool ortho_brute_force = false;
   bool ortho_dominance = true;   // per-tile dominance cull of the frame list (OrthoArgs::dominance); amb_ortho_set_dominance_cull(0) = plain list
 
@@ -296,12 +296,22 @@ int dsm_extract_halo(amb_ctx* ctx, const double* d_xyz, const unsigned long long
 int pcl_adaptive_prepare(amb_ctx* ctx, float** saved);
 int pcl_adaptive_finish(amb_ctx* ctx, int pass_status, const double* d_xyz, const unsigned long long* d_ids,
                         const int* d_intensities, size_t n, int32_t interpolation_radius, float* saved);
-struct JpegBands;  // jpeg_header.h
-// jpeg (host-frame path only, h_images == nullptr): the frames are JPEG files; the rows of each frame's bounding box of
-// winner pixels are decoded on the device in place of the rectangle copies (jpeg->row0 / row1 are filled here)
-int ortho_run(amb_ctx* ctx, const amb_camera* camera, const double* T_G_B, const uint8_t* const* d_images,
-              const uint8_t* const* h_images, size_t n, int32_t channels, size_t row_step, int32_t colored_ortho,
-              JpegBands* jpeg = nullptr);
+struct JpegFrame;  // jpeg_header.h
+// One OrthoBackwardGrid::process, wherever its frames live: checked by run_ortho (amb_api.cu), computed by ortho_run
+struct OrthoCall {
+  enum Frames { DEVICE, HOST, JPEG } frames = DEVICE;
+  const amb_camera* camera = nullptr;
+  const double* T_G_B = nullptr;           // [n][7]: x y z qw qx qy qz
+  size_t n = 0;
+  int32_t channels = 0;
+  size_t row_step = 0;                     // JPEG: set by run_ortho
+  int32_t colored_ortho = 0;
+  const uint8_t* const* images = nullptr;  // DEVICE: device rasters; HOST: host rasters
+  const void* const* files = nullptr;      // JPEG: the files and their sizes
+  const size_t* file_bytes = nullptr;
+  const JpegFrame* headers = nullptr;      // JPEG: parsed by run_ortho
+};
+int ortho_run(amb_ctx* ctx, const OrthoCall& call);
 // amb_comm.cu: one step of a sharded cloud on a context of a communicator of several ranks (halo exchange, then
 // dsm_run over the rank's points and the neighbours' halos); records the DSM events and sets dsm_timed itself
 int sharded_step(amb_ctx* ctx, const double* d_xyz, const int* d_intensities, const uint64_t* d_ids, size_t n_local,

@@ -971,60 +971,16 @@ double distortion_slope(const amb_camera& cam, double r) {
   return J * (1.0 + r);
 }
 
-}  // namespace
-
-// d_images != nullptr: frames resident in HBM -> one fused kernel per chunk of frames.
-// h_images != nullptr: frames in HOST memory -> phase A selects the winners without touching any pixel, the host
-//   reads back the per-frame bounding boxes of the winners' pixels, only those sub-rectangles are copied to the
-//   device (cudaMemcpy2DAsync), phase B fetches the texels.  Same results, a fraction of the PCIe traffic: a cell
-//   is seen by ~8 frames but takes its pixel from one.
-int ortho_run(amb_ctx* ctx, const amb_camera* camera, const double* T_G_B, const uint8_t* const* d_images,
-              const uint8_t* const* h_images, size_t n, int32_t channels, size_t row_step,
-              int32_t colored_ortho, JpegBands* jpeg) {
-  if (n == 0) return AMB_ERR_EMPTY;  // CHECK(!T_G_Bs.empty()), ortho-backward-grid.cc:225
-  if (!camera || !T_G_B || (!d_images && !h_images && !jpeg)) return AMB_ERR_INVALID_ARGUMENT;
-  const bool select_only = d_images == nullptr;
-  if (camera->width > 65535 || camera->height > 65535) return AMB_ERR_UNSUPPORTED;
-  if (colored_ortho ? channels != 3 : channels != 1) return AMB_ERR_SIZE_MISMATCH;
-  if (camera->width <= 0 || camera->height <= 0 || row_step < static_cast<size_t>(camera->width) * channels)
-    return AMB_ERR_SIZE_MISMATCH;
-  if (camera->dist_type < AMB_DIST_NONE || camera->dist_type > AMB_DIST_FOV) return AMB_ERR_UNSUPPORTED;
-  const int out_layer = colored_ortho ? AMB_LAYER_COLORED_ORTHO : AMB_LAYER_ORTHO;
-  const int need[4] = {AMB_LAYER_ELEVATION, AMB_LAYER_ELEVATION_ANGLE, AMB_LAYER_OBSERVATION_INDEX, out_layer};
-  // One fused launch (frames on the device, at most one chunk of them) writes every cell of the slab: when all three
-  // layers it writes are fresh, it stores their initial values itself instead of reading them after a fill.  Otherwise
-  // (host frames, several chunks, a layer an earlier call wrote) the layers are filled first and read as before.
-  bool fresh = !select_only && n <= static_cast<size_t>(kMaxFramesPerLaunch);
-  for (int k = 1; k < 4; ++k) fresh = fresh && layer_is_fresh(ctx, need[k]);
-  for (int l : need) {
-    bool overwritten = false;
-    const int st = fresh && l != AMB_LAYER_ELEVATION ? ensure_layer_overwrite(ctx, l, &overwritten) : ensure_layer(ctx, l);
-    if (st != AMB_OK) return st;
-    if (l != AMB_LAYER_ELEVATION) wait_layer_copy(ctx, l);  // written here; elevation is only read
-  }
-  const amb_geometry& g = ctx->geom;
-  cudaStream_t s = ctx->stream;
-
-  // T_G_C = T_G_B * T_C_B^-1 (ortho-backward-grid.cc:230-233), then the per-frame constants of
-  // X_c = T_G_C^-1 . X = R_C_G X - R_C_G t_G_C.
-  const Quat q_C_B = {camera->q_C_B[0], camera->q_C_B[1], camera->q_C_B[2], camera->q_C_B[3]};
+// T_G_C = T_G_B * T_C_B^-1 (ortho-backward-grid.cc:230-233), then the per-frame constants of
+// X_c = T_G_C^-1 . X = R_C_G X - R_C_G t_G_C, and the guards' scale with the inputs' magnitude (a->delta_coef, a->t_max).
+void frame_tables(const amb_camera& cam, const double* T_G_B, size_t n, FrameConst* fcs, double* cull, double* exact,
+                  OrthoArgs* a) {
+  const Quat q_C_B = {cam.q_C_B[0], cam.q_C_B[1], cam.q_C_B[2], cam.q_C_B[3]};
   const Quat q_B_C = {q_C_B.w, -q_C_B.x, -q_C_B.y, -q_C_B.z};
-  const V3 t_C_B = {camera->t_C_B[0], camera->t_C_B[1], camera->t_C_B[2]};
+  const V3 t_C_B = {cam.t_C_B[0], cam.t_C_B[1], cam.t_C_B[2]};
   const V3 r_tmp = qrot(q_B_C, t_C_B);
   const V3 t_B_C = {-r_tmp.x, -r_tmp.y, -r_tmp.z};
-  // per-call tables live in pinned staging (see HostStage); the previous call's copies must have left it
-  const int turn = static_cast<int>(ctx->stage_turn++ & 1u);
-  HostStage& stage = ctx->stages[turn];
-  cudaEvent_t& stage_event = ctx->stage_events[turn];
-  if (!stage_event) AMB_CUDA(ctx, cudaEventCreateWithFlags(&stage_event, cudaEventDisableTiming));
-  AMB_CUDA(ctx, cudaEventSynchronize(stage_event));   // the call before the previous one: long finished in practice
-  AMB_CUDA(ctx, stage.reserve(n * (sizeof(FrameConst) + 20 * sizeof(double) + 8 * sizeof(int) +
-                                        sizeof(FrameRect) + sizeof(uint8_t*)) + 1024));
-  stage.used = 0;
-  FrameConst* fcs = stage.take<FrameConst>(n);
-  double* cull = stage.take<double>(12 * n);
-  double* exact = stage.take<double>(8 * n);
-  double q_norm2 = 1.0, t_max = 0.0;   // magnitudes the guards scale with (kDeltaUlps)
+  double q_norm2 = 1.0, t_max = 0.0;
   for (size_t f = 0; f < n; ++f) {
     const double* p = T_G_B + 7 * f;
     const Quat q_G_B = {p[3], p[4], p[5], p[6]};
@@ -1052,136 +1008,86 @@ int ortho_run(amb_ctx* ctx, const amb_camera* camera, const double* T_G_B, const
     t_max = std::max({t_max, std::fabs(t.x), std::fabs(t.y), std::fabs(t.z), std::fabs(ti.x), std::fabs(ti.y),
                       std::fabs(ti.z)});
   }
+  a->delta_coef = kDeltaUlps * std::ldexp(1.0, -53) * q_norm2;
+  a->t_max = t_max;
+}
 
-  AMB_CUDA(ctx, ctx->frame_table.reserve(n * sizeof(uint8_t*)));
-  {
-    const int cst = ensure_counters(ctx);  // born zeroed; the CHECK(alpha > 0) flag is sticky until reported
-    if (cst != AMB_OK) return cst;
-  }
-  unsigned int* counters = ctx->counters.as<unsigned int>();
-  if (!select_only) {
-    const uint8_t** table = stage.take<const uint8_t*>(n);
-    for (size_t f = 0; f < n; ++f) table[f] = d_images[f];
-    AMB_CUDA(ctx, cudaMemcpyAsync(ctx->frame_table.ptr, table, n * sizeof(uint8_t*), cudaMemcpyHostToDevice, s));
-  }
-  AMB_CUDA(ctx, ctx->frame_cull.reserve(20 * n * sizeof(double)));   // [12 n cull | 8 n exact]
-  AMB_CUDA(ctx, cudaMemcpyAsync(ctx->frame_cull.ptr, cull, 12 * n * sizeof(double), cudaMemcpyHostToDevice, s));
-  AMB_CUDA(ctx, cudaMemcpyAsync(ctx->frame_cull.as<double>() + 12 * n, exact, 8 * n * sizeof(double),
-                                cudaMemcpyHostToDevice, s));
-
-  OrthoArgs a;
-  std::memset(&a, 0, sizeof(a));
-  a.elevation = ctx->layers[AMB_LAYER_ELEVATION];
-  a.elevation_angle = ctx->layers[AMB_LAYER_ELEVATION_ANGLE];
-  a.observation_index = ctx->layers[AMB_LAYER_OBSERVATION_INDEX];
-  a.out_layer = ctx->layers[out_layer];
-  a.error_flag = counters + CTR_ORTHO_CHECK;
-  int* bbox = nullptr;      // pinned: initial values up, results back
-  int* bbox_back = nullptr;
-  const size_t cells = ctx->slab_cells();
-  if (select_only) {
-    AMB_CUDA(ctx, ctx->ortho_pix.reserve(cells * sizeof(unsigned int)));
-    AMB_CUDA(ctx, ctx->ortho_bbox.reserve(n * 4 * sizeof(int)));
-    AMB_CUDA(ctx, cudaMemsetAsync(ctx->ortho_pix.ptr, 0xff, cells * sizeof(unsigned int), s));
-    bbox = stage.take<int>(4 * n);
-    bbox_back = stage.take<int>(4 * n);
-    for (size_t f = 0; f < n; ++f) {
-      bbox[4 * f + 0] = bbox[4 * f + 1] = 0x7fffffff;
-      bbox[4 * f + 2] = bbox[4 * f + 3] = -1;
-    }
-    AMB_CUDA(ctx, cudaMemcpyAsync(ctx->ortho_bbox.ptr, bbox, 4 * n * sizeof(int), cudaMemcpyHostToDevice, s));
-    a.pix = ctx->ortho_pix.as<unsigned int>();
-    a.bbox = ctx->ortho_bbox.as<int>();
-  }
-  a.row_step = row_step;
-  a.rows = g.rows;
-  a.cols_slab = ctx->col_end - ctx->col_begin;
-  a.col_begin = ctx->col_begin;
-  a.width = camera->width;
-  a.height = camera->height;
-  a.channels = channels;
-  a.colored = colored_ortho ? 1 : 0;
-  a.dist_type = camera->dist_type;
-  a.base_x = g.pos_x + (0.5 * g.length_x - 0.5 * g.resolution);
-  a.base_y = g.pos_y + (0.5 * g.length_y - 0.5 * g.resolution);
-  a.res = g.resolution;
-  a.fu = camera->fu; a.fv = camera->fv; a.cu = camera->cu; a.cv = camera->cv;
-  a.d0 = camera->dist[0]; a.d1 = camera->dist[1]; a.d2 = camera->dist[2]; a.d3 = camera->dist[3];
-  if (camera->dist_type == AMB_DIST_FOV) a.d1 = std::tan(camera->dist[0] / 2.);  // FOV: the kernels take tan(w/2) from here
-  a.do_cull = ctx->ortho_brute_force ? 0 : 1;
+// The camera's cull bounds (the fields of `a` from `cone` to the dominance cull's) and px_coef.  `cull`: not brute force.
+void camera_bounds(const amb_camera& cam, bool cull, bool dominance, OrthoArgs* a) {
   double cc = 0.0, sc = 1.0, tc = 0.0;
-  a.cone = compute_view_cone(*camera, &cc, &sc, &tc) ? 1 : 0;
-  a.cos_c = cc;
-  a.sin_c = sc;
-  a.rect = 0;
-  if (a.cone && compute_view_rect(*camera, tc, &a.u_lo, &a.u_hi, &a.v_lo, &a.v_hi)) {
-    a.rect = 1;
-    a.nu_lo = std::sqrt(1.0 + a.u_lo * a.u_lo);
-    a.nu_hi = std::sqrt(1.0 + a.u_hi * a.u_hi);
-    a.nv_lo = std::sqrt(1.0 + a.v_lo * a.v_lo);
-    a.nv_hi = std::sqrt(1.0 + a.v_hi * a.v_hi);
+  a->cone = compute_view_cone(cam, &cc, &sc, &tc) ? 1 : 0;
+  a->cos_c = cc;
+  a->sin_c = sc;
+  a->rect = 0;
+  if (a->cone && compute_view_rect(cam, tc, &a->u_lo, &a->u_hi, &a->v_lo, &a->v_hi)) {
+    a->rect = 1;
+    a->nu_lo = std::sqrt(1.0 + a->u_lo * a->u_lo);
+    a->nu_hi = std::sqrt(1.0 + a->u_hi * a->u_hi);
+    a->nv_lo = std::sqrt(1.0 + a->v_lo * a->v_lo);
+    a->nv_hi = std::sqrt(1.0 + a->v_hi * a->v_hi);
   }
-  // guards scaled with the inputs' magnitude; without a view cone the normalised radius of an imaged ray is bounded by
-  // nothing better than the cone scan's limit
-  a.delta_coef = kDeltaUlps * std::ldexp(1.0, -53) * q_norm2;
-  a.t_max = t_max;
-  a.px_coef = std::max(std::fabs(camera->fu), std::fabs(camera->fv)) * distortion_slope(*camera, a.cone ? tc : 1.0e3);
+  // without a view cone the normalised radius of an imaged ray is bounded by nothing better than the cone scan's limit
+  a->px_coef = std::max(std::fabs(cam.fu), std::fabs(cam.fv)) * distortion_slope(cam, a->cone ? tc : 1.0e3);
 
-  // Dominance cull (amb_ortho_set_dominance_cull): needs an INNER bound, a set of rays that are certainly imaged inside
-  // the raster.  r_in: normalised distance from the principal point to the nearest raster edge.
-  if (ctx->ortho_dominance && a.do_cull && a.cone && camera->fu > 0.0 && camera->fv > 0.0) {
-    const double r_in = std::min(std::min(camera->cu, camera->width - camera->cu) / camera->fu,
-                                 std::min(camera->cv, camera->height - camera->cv) / camera->fv) * (1.0 - 1e-9);
-    bool inner = false;
-    double th = 0.0;  // inner view cone (equidistant, FOV): every ray with angle-to-axis below th is imaged
-    if (a.rect) {
-      // Pinhole / rad-tan: the INNER rectangle, the raster's normalised extent shrunk by the same distortion bound E the
-      // outer rectangle was grown by: a ray with an undistorted keypoint inside it is imaged inside the raster.
-      const double E_u = a.u_hi - (camera->width - camera->cu) / camera->fu;   // what compute_view_rect added
-      const double E_v = a.v_hi - (camera->height - camera->cv) / camera->fv;
-      const double E = std::max(E_u, E_v) * (1.0 + 1e-9) + 1e-9;
-      a.ui_lo = -camera->cu / camera->fu + E;
-      a.ui_hi = (camera->width - camera->cu) / camera->fu - E;
-      a.vi_lo = -camera->cv / camera->fv + E;
-      a.vi_hi = (camera->height - camera->cv) / camera->fv - E;
-      a.nui_lo = std::sqrt(1.0 + a.ui_lo * a.ui_lo);
-      a.nui_hi = std::sqrt(1.0 + a.ui_hi * a.ui_hi);
-      a.nvi_lo = std::sqrt(1.0 + a.vi_lo * a.vi_lo);
-      a.nvi_hi = std::sqrt(1.0 + a.vi_hi * a.vi_hi);
-      inner = a.ui_lo < a.ui_hi && a.vi_lo < a.vi_hi;
-    } else if (a.dist_type == AMB_DIST_EQUIDISTANT) {
-      // Equidistant: the keypoint's distance from the principal point (normalised) is |theta * poly(theta^2)| whatever
-      // the azimuth, so every ray with theta <= th is imaged if that radius stays below r_in on [0, th].  Scan outwards
-      // with a Lipschitz bound on the radius; stop at the first step that might leave the inscribed circle.
-      const double* k = camera->dist;
-      const double step = 1e-4;
-      while (th < 1.5) {
-        const double b = th + step, b2 = b * b;
-        const double lip = 1.0 + 3.0 * std::fabs(k[0]) * b2 + 5.0 * std::fabs(k[1]) * b2 * b2 +
-                           7.0 * std::fabs(k[2]) * b2 * b2 * b2 + 9.0 * std::fabs(k[3]) * b2 * b2 * b2 * b2;  // >= |dr/dtheta|
-        const double t2 = th * th;
-        const double r_th = std::fabs(th * (1.0 + k[0] * t2 + k[1] * t2 * t2 + k[2] * t2 * t2 * t2 + k[3] * t2 * t2 * t2 * t2));
-        if (r_th + lip * step >= r_in) break;
-        th = b;
-      }
-      inner = th > 1e-3;
-    } else if (a.dist_type == AMB_DIST_FOV) {
-      // FOV: radius atan(2 tan(w/2) tan(theta)) / w, increasing — every ray with that radius below r_in is imaged:
-      // tan(th) = tan(w r_in) / (2 tan(w/2))
-      const double w = std::fabs(camera->dist[0]);
-      double tan_in = r_in;
-      if (w * w >= 1e-5) tan_in = (w * r_in < 1.5) ? std::tan(w * r_in) / (2.0 * std::fabs(std::tan(w / 2.))) : -1.0;
-      th = tan_in > 0.0 ? std::atan(tan_in) * (1.0 - 1e-9) : 0.0;
-      inner = th > 1e-3;
+  // Dominance cull: needs an INNER bound, a set of rays that are certainly imaged inside the raster.  r_in: normalised
+  // distance from the principal point to the nearest raster edge.
+  if (!(dominance && cull && a->cone && cam.fu > 0.0 && cam.fv > 0.0)) return;
+  const double r_in = std::min(std::min(cam.cu, cam.width - cam.cu) / cam.fu,
+                               std::min(cam.cv, cam.height - cam.cv) / cam.fv) * (1.0 - 1e-9);
+  bool inner = false;
+  double th = 0.0;  // inner view cone (equidistant, FOV): every ray with angle-to-axis below th is imaged
+  if (a->rect) {
+    // Pinhole / rad-tan: the INNER rectangle, the raster's normalised extent shrunk by the same distortion bound E the
+    // outer rectangle was grown by: a ray with an undistorted keypoint inside it is imaged inside the raster.
+    const double E_u = a->u_hi - (cam.width - cam.cu) / cam.fu;   // what compute_view_rect added
+    const double E_v = a->v_hi - (cam.height - cam.cv) / cam.fv;
+    const double E = std::max(E_u, E_v) * (1.0 + 1e-9) + 1e-9;
+    a->ui_lo = -cam.cu / cam.fu + E;
+    a->ui_hi = (cam.width - cam.cu) / cam.fu - E;
+    a->vi_lo = -cam.cv / cam.fv + E;
+    a->vi_hi = (cam.height - cam.cv) / cam.fv - E;
+    a->nui_lo = std::sqrt(1.0 + a->ui_lo * a->ui_lo);
+    a->nui_hi = std::sqrt(1.0 + a->ui_hi * a->ui_hi);
+    a->nvi_lo = std::sqrt(1.0 + a->vi_lo * a->vi_lo);
+    a->nvi_hi = std::sqrt(1.0 + a->vi_hi * a->vi_hi);
+    inner = a->ui_lo < a->ui_hi && a->vi_lo < a->vi_hi;
+  } else if (cam.dist_type == AMB_DIST_EQUIDISTANT) {
+    // Equidistant: the keypoint's distance from the principal point (normalised) is |theta * poly(theta^2)| whatever
+    // the azimuth, so every ray with theta <= th is imaged if that radius stays below r_in on [0, th].  Scan outwards
+    // with a Lipschitz bound on the radius; stop at the first step that might leave the inscribed circle.
+    const double* k = cam.dist;
+    const double step = 1e-4;
+    while (th < 1.5) {
+      const double b = th + step, b2 = b * b;
+      const double lip = 1.0 + 3.0 * std::fabs(k[0]) * b2 + 5.0 * std::fabs(k[1]) * b2 * b2 +
+                         7.0 * std::fabs(k[2]) * b2 * b2 * b2 + 9.0 * std::fabs(k[3]) * b2 * b2 * b2 * b2;  // >= |dr/dtheta|
+      const double t2 = th * th;
+      const double r_th = std::fabs(th * (1.0 + k[0] * t2 + k[1] * t2 * t2 + k[2] * t2 * t2 * t2 + k[3] * t2 * t2 * t2 * t2));
+      if (r_th + lip * step >= r_in) break;
+      th = b;
     }
-    if (inner) {
-      const double margin = 1e-4;  // rad; the float32 rounding of an angle <= pi/2 is < 1.2e-7
-      a.dominance = 1;
-      a.dom_cos_in = std::cos(th);
-      a.dom_cos_margin = std::cos(margin);
-      a.dom_sin_margin = std::sin(margin);
-    }
+    inner = th > 1e-3;
+  } else if (cam.dist_type == AMB_DIST_FOV) {
+    // FOV: radius atan(2 tan(w/2) tan(theta)) / w, increasing — every ray with that radius below r_in is imaged:
+    // tan(th) = tan(w r_in) / (2 tan(w/2))
+    const double w = std::fabs(cam.dist[0]);
+    double tan_in = r_in;
+    if (w * w >= 1e-5) tan_in = (w * r_in < 1.5) ? std::tan(w * r_in) / (2.0 * std::fabs(std::tan(w / 2.))) : -1.0;
+    th = tan_in > 0.0 ? std::atan(tan_in) * (1.0 - 1e-9) : 0.0;
+    inner = th > 1e-3;
   }
+  if (inner) {
+    const double margin = 1e-4;  // rad; the float32 rounding of an angle <= pi/2 is < 1.2e-7
+    a->dominance = 1;
+    a->dom_cos_in = std::cos(th);
+    a->dom_cos_margin = std::cos(margin);
+    a->dom_sin_margin = std::sin(margin);
+  }
+}
+
+// One launch per chunk of frames, whose constants take their turn in c_frames (ConstantGuard).
+int launch_chunks(amb_ctx* ctx, OrthoArgs& a, const FrameConst* fcs, size_t n, bool select_only, bool fresh) {
+  cudaStream_t s = ctx->stream;
   const int tiles_i = (a.rows + OTI - 1) / OTI, tiles_j = (a.cols_slab + OTJ - 1) / OTJ;
   ctx->ortho_launches = 0;
   for (size_t f0 = 0; f0 < n; f0 += kMaxFramesPerLaunch) {  // ascending chunks keep the frame order
@@ -1208,92 +1114,183 @@ int ortho_run(amb_ctx* ctx, const amb_camera* camera, const double* T_G_B, const
     AMB_CUDA(ctx, cudaEventRecord(guard_event, s));
   }
   AMB_CUDA(ctx, cudaGetLastError());
-  ctx->ortho_h2d_bytes = 0;
-  // elevation_angle and observation_index are final here: start streaming them to their host mirrors
-  int mst = mirror_layer(ctx, AMB_LAYER_ELEVATION_ANGLE);
-  if (mst == AMB_OK) mst = mirror_layer(ctx, AMB_LAYER_OBSERVATION_INDEX);
-  if (mst != AMB_OK) return mst;
-  if (!select_only) {
-    AMB_CUDA(ctx, cudaEventRecord(stage_event, s));
-    return mirror_layer(ctx, out_layer);
-  }
+  return AMB_OK;
+}
 
-  // ---- host frames: bounding boxes back, sub-rectangles up, texel gather ----
+// The two texel sources of host frames fill the FrameRect table and ctx->ortho_h2d_bytes from the per-frame bounding
+// boxes of the winners' pixels.  Rasters: the sub-rectangle of each frame's box is copied to the device.
+int rect_source(amb_ctx* ctx, const OrthoCall& c, const int* bbox, FrameRect* rects) {
+  // bytes per row and rows of frame f's box; the rows of its device copy are 256-byte aligned
+  auto row_bytes = [&](size_t f) { return static_cast<size_t>(bbox[4 * f + 2] - bbox[4 * f + 0] + 1) * c.channels; };
+  auto rows = [&](size_t f) { return static_cast<size_t>(bbox[4 * f + 3] - bbox[4 * f + 1] + 1); };
+  auto pitch = [&](size_t f) { return (row_bytes(f) + 255) & ~static_cast<size_t>(255); };
+  size_t total = 0;
+  for (size_t f = 0; f < c.n; ++f)
+    if (bbox[4 * f + 2] >= 0) total += pitch(f) * rows(f);  // xmax < 0: no cell takes its pixel from this frame
+  AMB_CUDA(ctx, ctx->frames.reserve(total + 256));
+  uint8_t* dst = ctx->frames.as<uint8_t>();
+  std::vector<StagedRect> copies;
+  copies.reserve(c.n);
+  for (size_t f = 0; f < c.n; ++f) {
+    rects[f] = FrameRect{nullptr, 0, 0, 0, 0};
+    if (bbox[4 * f + 2] < 0) continue;
+    const int x0 = bbox[4 * f + 0], y0 = bbox[4 * f + 1];
+    rects[f] = FrameRect{dst, x0, y0, static_cast<int>(pitch(f)), 0};
+    const uint8_t* src = c.images[f] + static_cast<size_t>(y0) * c.row_step + static_cast<size_t>(x0) * c.channels;
+    // (frames in pageable memory — cv::Mat storage — are packed into pinned slots by the worker pool: host_staging.cu)
+    copies.push_back(StagedRect{dst, pitch(f), src, c.row_step, row_bytes(f), rows(f)});
+    ctx->ortho_h2d_bytes += static_cast<int64_t>(row_bytes(f) * rows(f));
+    dst += pitch(f) * rows(f);
+  }
+  return staged_h2d_rects(ctx, copies.data(), copies.size(), ctx->stream);
+}
+
+// JPEG files: the rows of each frame's box, every column, decoded on the device (frames without a winner are neither
+// copied nor decoded)
+int jpeg_source(amb_ctx* ctx, const OrthoCall& c, const int* bbox, FrameRect* rects) {
+  const size_t n = c.n;
+  std::vector<int32_t> row0(n), row1(n);
+  std::vector<unsigned char*> ptr(n);
+  std::vector<int> pitch(n);
+  for (size_t f = 0; f < n; ++f) {
+    row0[f] = bbox[4 * f + 2] < 0 ? 0 : bbox[4 * f + 1];
+    row1[f] = bbox[4 * f + 2] < 0 ? 0 : bbox[4 * f + 3] + 1;
+  }
+  const JpegBands bands{c.files, c.file_bytes, c.headers, row0.data(), row1.data(), n, c.channels};
+  const int st = jpeg_decode_bands(ctx, bands, ptr.data(), pitch.data());
+  if (st != AMB_OK) return st;
+  for (size_t f = 0; f < n; ++f) {
+    rects[f] = FrameRect{ptr[f], 0, row0[f], pitch[f], 0};
+    if (ptr[f]) ctx->ortho_h2d_bytes += static_cast<int64_t>(c.file_bytes[f]);
+  }
+  return AMB_OK;
+}
+
+// ---- host frames: bounding boxes back, texels up from their source, texel gather ----
+int host_frames_texels(amb_ctx* ctx, const OrthoCall& c, const OrthoArgs& a, HostStage& stage, int* bbox) {
+  cudaStream_t s = ctx->stream;
   AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_ORTHO_SELECT_END], s));
-  {
-    int* mapped = nullptr;
-    AMB_CUDA(ctx, cudaHostGetDevicePointer(reinterpret_cast<void**>(&mapped), bbox_back, 0));
-    copy_to_mapped_kernel<<<8, 256, 0, s>>>(ctx->ortho_bbox.as<int>(), mapped, static_cast<int>(4 * n));
-  }
+  ctx->ortho_h2d_bytes = 0;
+  int* mapped = nullptr;
+  AMB_CUDA(ctx, cudaHostGetDevicePointer(reinterpret_cast<void**>(&mapped), bbox, 0));
+  copy_to_mapped_kernel<<<8, 256, 0, s>>>(ctx->ortho_bbox.as<int>(), mapped, static_cast<int>(4 * c.n));
   AMB_CUDA(ctx, cudaStreamSynchronize(s));
-  bbox = bbox_back;
-  FrameRect* rects = stage.take<FrameRect>(n);
-  AMB_CUDA(ctx, ctx->frame_rects.reserve(n * sizeof(FrameRect)));
-  if (jpeg) {
-    // JPEG frames: the rows of each frame's box, every column, decoded on the device (frames without a winner are
-    // neither copied nor decoded)
-    std::vector<int32_t> row0(n), row1(n);
-    std::vector<unsigned char*> ptr(n);
-    std::vector<int> pitch(n);
-    for (size_t f = 0; f < n; ++f) {
-      row0[f] = bbox[4 * f + 2] < 0 ? 0 : bbox[4 * f + 1];
-      row1[f] = bbox[4 * f + 2] < 0 ? 0 : bbox[4 * f + 3] + 1;
-    }
-    jpeg->row0 = row0.data();
-    jpeg->row1 = row1.data();
-    const int dst = jpeg_decode_bands(ctx, *jpeg, ptr.data(), pitch.data());
-    if (dst != AMB_OK) return dst;
-    for (size_t f = 0; f < n; ++f) {
-      rects[f].ptr = ptr[f];
-      rects[f].x0 = 0;
-      rects[f].y0 = row0[f];
-      rects[f].pitch = pitch[f];
-      rects[f].pad_ = 0;
-      if (ptr[f]) ctx->ortho_h2d_bytes += static_cast<int64_t>(jpeg->file_bytes[f]);
-    }
-  } else {
-    size_t total = 0;
-    for (size_t f = 0; f < n; ++f) {
-      FrameRect& r = rects[f];
-      r.ptr = nullptr;
-      r.x0 = r.y0 = r.pitch = r.pad_ = 0;
-      if (bbox[4 * f + 2] < 0) continue;  // no cell takes its pixel from this frame
-      const int w = bbox[4 * f + 2] - bbox[4 * f + 0] + 1;
-      r.x0 = bbox[4 * f + 0];
-      r.y0 = bbox[4 * f + 1];
-      r.pitch = static_cast<int>((static_cast<size_t>(w) * channels + 255) & ~static_cast<size_t>(255));
-      r.pad_ = bbox[4 * f + 3] - bbox[4 * f + 1] + 1;  // rows
-      total += static_cast<size_t>(r.pitch) * r.pad_;
-    }
-    AMB_CUDA(ctx, ctx->frames.reserve(total + 256));
-    size_t off = 0;
-    std::vector<StagedRect> copies;
-    copies.reserve(n);
-    for (size_t f = 0; f < n; ++f) {
-      FrameRect& r = rects[f];
-      if (bbox[4 * f + 2] < 0) continue;
-      const int w = bbox[4 * f + 2] - r.x0 + 1, h = r.pad_;
-      uint8_t* dst = ctx->frames.as<uint8_t>() + off;
-      const uint8_t* src = h_images[f] + static_cast<size_t>(r.y0) * row_step + static_cast<size_t>(r.x0) * channels;
-      // (frames in pageable memory — cv::Mat storage — are packed into pinned slots by the worker pool: host_staging.cu)
-      copies.push_back(StagedRect{dst, static_cast<size_t>(r.pitch), src, row_step, static_cast<size_t>(w) * channels,
-                                  static_cast<size_t>(h)});
-      ctx->ortho_h2d_bytes += static_cast<int64_t>(w) * channels * h;
-      r.ptr = dst;
-      off += static_cast<size_t>(r.pitch) * h;
-      r.pad_ = 0;
-    }
-    {
-      const int cst = staged_h2d_rects(ctx, copies.data(), copies.size(), s);
-      if (cst != AMB_OK) return cst;
-    }
-  }
-  AMB_CUDA(ctx, cudaMemcpyAsync(ctx->frame_rects.ptr, rects, n * sizeof(FrameRect), cudaMemcpyHostToDevice, s));
+  FrameRect* rects = stage.take<FrameRect>(c.n);
+  AMB_CUDA(ctx, ctx->frame_rects.reserve(c.n * sizeof(FrameRect)));
+  const int st = c.frames == OrthoCall::JPEG ? jpeg_source(ctx, c, bbox, rects) : rect_source(ctx, c, bbox, rects);
+  if (st != AMB_OK) return st;
+  AMB_CUDA(ctx, cudaMemcpyAsync(ctx->frame_rects.ptr, rects, c.n * sizeof(FrameRect), cudaMemcpyHostToDevice, s));
   AMB_CUDA(ctx, cudaEventRecord(ctx->events[EV_ORTHO_COPY_END], s));
   ortho_texel_kernel<<<ctx->num_sms * 8, 256, 0, s>>>(a.pix, a.observation_index, ctx->frame_rects.as<FrameRect>(),
-                                                    a.out_layer, cells, channels, a.colored);
+                                                    a.out_layer, ctx->slab_cells(), c.channels, a.colored);
   ctx->ortho_launches += 1;
   AMB_CUDA(ctx, cudaGetLastError());
+  return AMB_OK;
+}
+
+}  // namespace
+
+// Device frames: one fused kernel per chunk of frames.
+// Host and JPEG frames: phase A selects the winners without touching any pixel, the host reads back the per-frame
+// bounding boxes of the winners' pixels, only those parts of the frames reach the device, phase B fetches the texels.
+// Same results, a fraction of the PCIe traffic: a cell is seen by ~8 frames but takes its pixel from one.
+int ortho_run(amb_ctx* ctx, const OrthoCall& c) {
+  const amb_camera& cam = *c.camera;
+  const size_t n = c.n;
+  const bool select_only = c.frames != OrthoCall::DEVICE;
+  const int out_layer = c.colored_ortho ? AMB_LAYER_COLORED_ORTHO : AMB_LAYER_ORTHO;
+  const int need[4] = {AMB_LAYER_ELEVATION, AMB_LAYER_ELEVATION_ANGLE, AMB_LAYER_OBSERVATION_INDEX, out_layer};
+  // One fused launch (frames on the device, at most one chunk of them) writes every cell of the slab: when all three
+  // layers it writes are fresh, it stores their initial values itself instead of reading them after a fill.  Otherwise
+  // (host frames, several chunks, a layer an earlier call wrote) the layers are filled first and read as before.
+  bool fresh = !select_only && n <= static_cast<size_t>(kMaxFramesPerLaunch);
+  for (int k = 1; k < 4; ++k) fresh = fresh && layer_is_fresh(ctx, need[k]);
+  for (int l : need) {
+    bool overwritten = false;
+    const int st = fresh && l != AMB_LAYER_ELEVATION ? ensure_layer_overwrite(ctx, l, &overwritten) : ensure_layer(ctx, l);
+    if (st != AMB_OK) return st;
+    if (l != AMB_LAYER_ELEVATION) wait_layer_copy(ctx, l);  // written here; elevation is only read
+  }
+  const amb_geometry& g = ctx->geom;
+  cudaStream_t s = ctx->stream;
+
+  // per-call tables live in pinned staging (see HostStage); the previous call's copies must have left it
+  const int turn = static_cast<int>(ctx->stage_turn++ & 1u);
+  HostStage& stage = ctx->stages[turn];
+  cudaEvent_t& stage_event = ctx->stage_events[turn];
+  if (!stage_event) AMB_CUDA(ctx, cudaEventCreateWithFlags(&stage_event, cudaEventDisableTiming));
+  AMB_CUDA(ctx, cudaEventSynchronize(stage_event));   // the call before the previous one: long finished in practice
+  AMB_CUDA(ctx, stage.reserve(n * (sizeof(FrameConst) + 20 * sizeof(double) + 8 * sizeof(int) +
+                                        sizeof(FrameRect) + sizeof(uint8_t*)) + 1024));
+  stage.used = 0;
+  FrameConst* fcs = stage.take<FrameConst>(n);
+  double* cull = stage.take<double>(12 * n);
+  double* exact = stage.take<double>(8 * n);
+  OrthoArgs a;
+  std::memset(&a, 0, sizeof(a));
+  frame_tables(cam, c.T_G_B, n, fcs, cull, exact, &a);
+
+  AMB_CUDA(ctx, ctx->frame_table.reserve(n * sizeof(uint8_t*)));
+  {
+    const int cst = ensure_counters(ctx);  // born zeroed; the CHECK(alpha > 0) flag is sticky until reported
+    if (cst != AMB_OK) return cst;
+  }
+  unsigned int* counters = ctx->counters.as<unsigned int>();
+  if (!select_only) {
+    const uint8_t** table = stage.take<const uint8_t*>(n);
+    for (size_t f = 0; f < n; ++f) table[f] = c.images[f];
+    AMB_CUDA(ctx, cudaMemcpyAsync(ctx->frame_table.ptr, table, n * sizeof(uint8_t*), cudaMemcpyHostToDevice, s));
+  }
+  AMB_CUDA(ctx, ctx->frame_cull.reserve(20 * n * sizeof(double)));   // [12 n cull | 8 n exact]
+  AMB_CUDA(ctx, cudaMemcpyAsync(ctx->frame_cull.ptr, cull, 12 * n * sizeof(double), cudaMemcpyHostToDevice, s));
+  AMB_CUDA(ctx, cudaMemcpyAsync(ctx->frame_cull.as<double>() + 12 * n, exact, 8 * n * sizeof(double),
+                                cudaMemcpyHostToDevice, s));
+
+  a.elevation = ctx->layers[AMB_LAYER_ELEVATION];
+  a.elevation_angle = ctx->layers[AMB_LAYER_ELEVATION_ANGLE];
+  a.observation_index = ctx->layers[AMB_LAYER_OBSERVATION_INDEX];
+  a.out_layer = ctx->layers[out_layer];
+  a.error_flag = counters + CTR_ORTHO_CHECK;
+  int* bbox_back = nullptr;  // pinned and mapped: the select kernel's bounding boxes come back here
+  if (select_only) {
+    const size_t cells = ctx->slab_cells();
+    AMB_CUDA(ctx, ctx->ortho_pix.reserve(cells * sizeof(unsigned int)));
+    AMB_CUDA(ctx, ctx->ortho_bbox.reserve(n * 4 * sizeof(int)));
+    AMB_CUDA(ctx, cudaMemsetAsync(ctx->ortho_pix.ptr, 0xff, cells * sizeof(unsigned int), s));
+    int* bbox = stage.take<int>(4 * n);
+    bbox_back = stage.take<int>(4 * n);
+    for (size_t f = 0; f < n; ++f) {
+      bbox[4 * f + 0] = bbox[4 * f + 1] = 0x7fffffff;
+      bbox[4 * f + 2] = bbox[4 * f + 3] = -1;
+    }
+    AMB_CUDA(ctx, cudaMemcpyAsync(ctx->ortho_bbox.ptr, bbox, 4 * n * sizeof(int), cudaMemcpyHostToDevice, s));
+    a.pix = ctx->ortho_pix.as<unsigned int>();
+    a.bbox = ctx->ortho_bbox.as<int>();
+  }
+  a.row_step = c.row_step;
+  a.rows = g.rows;
+  a.cols_slab = ctx->col_end - ctx->col_begin;
+  a.col_begin = ctx->col_begin;
+  a.width = cam.width;
+  a.height = cam.height;
+  a.channels = c.channels;
+  a.colored = c.colored_ortho ? 1 : 0;
+  a.dist_type = cam.dist_type;
+  a.base_x = g.pos_x + (0.5 * g.length_x - 0.5 * g.resolution);
+  a.base_y = g.pos_y + (0.5 * g.length_y - 0.5 * g.resolution);
+  a.res = g.resolution;
+  a.fu = cam.fu; a.fv = cam.fv; a.cu = cam.cu; a.cv = cam.cv;
+  a.d0 = cam.dist[0]; a.d1 = cam.dist[1]; a.d2 = cam.dist[2]; a.d3 = cam.dist[3];
+  if (cam.dist_type == AMB_DIST_FOV) a.d1 = std::tan(cam.dist[0] / 2.);  // FOV: the kernels take tan(w/2) from here
+  a.do_cull = ctx->ortho_brute_force ? 0 : 1;
+  camera_bounds(cam, a.do_cull != 0, ctx->ortho_dominance, &a);
+
+  int st = launch_chunks(ctx, a, fcs, n, select_only, fresh);
+  // elevation_angle and observation_index are final here: start streaming them to their host mirrors
+  if (st == AMB_OK) st = mirror_layer(ctx, AMB_LAYER_ELEVATION_ANGLE);
+  if (st == AMB_OK) st = mirror_layer(ctx, AMB_LAYER_OBSERVATION_INDEX);
+  if (st == AMB_OK && select_only) st = host_frames_texels(ctx, c, a, stage, bbox_back);
+  if (st != AMB_OK) return st;
   AMB_CUDA(ctx, cudaEventRecord(stage_event, s));
   return mirror_layer(ctx, out_layer);
 }

@@ -40,7 +40,8 @@ def test_variant_gpu_tests_pass_on_the_emulated_kernels(sched):
     # result depended on who runs first (e.g. a missing barrier between a write and another thread's read) would differ
     tail = run_child("gpu", ["test_gpu_ortho_dominance.py", "test_gpu_compact_mirrors.py", "test_ortho_from_pcl.py",
                              "test_stereo_rectify.py", "test_gpu_dsm_adversarial.py", "test_gpu_dsm_heights.py",
-                             "test_gpu_dsm_binning.py", "test_gpu_stereo_device.py", "test_gpu_cloud_entry_points.py"],
+                             "test_gpu_dsm_binning.py", "test_gpu_stereo_device.py", "test_gpu_cloud_entry_points.py",
+                             "test_gpu_ortho_entry_points.py"],
                      sched=sched)
     assert " passed" in tail and "failed" not in tail
 
@@ -49,7 +50,7 @@ def test_validated_gpu_tests_pass_on_the_emulated_kernels_too():
     # everything except the tests that create their inputs on a real device with torch.cuda
     tail = run_child("gpu", ["test_gpu_smoke.py", "test_gpu_refsrc.py", "test_stereo_reproject.py", "test_gpu_dsm.py",
                              "test_gpu_ortho.py", "test_ortho_from_pcl.py", "test_gpu_dsm_adversarial.py",
-                             "test_gpu_dsm_heights.py", "test_gpu_cloud_entry_points.py"],
+                             "test_gpu_dsm_heights.py", "test_gpu_cloud_entry_points.py", "test_gpu_ortho_entry_points.py"],
                      extra=["-k", "not large and not full_baseline_size"])
     assert " passed" in tail and "failed" not in tail
     import re
