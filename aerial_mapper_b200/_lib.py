@@ -174,6 +174,16 @@ SYMBOLS = {
     "amb_cog_tiles_device": (C.c_int, [_P, _P, C.c_int32, C.c_int32, C.c_size_t, C.c_int, C.c_int32, _P, C.c_size_t,
                                        C.POINTER(C.c_size_t), _P]),
     "amb_export_cog_tiles": (C.c_int, [_P, C.c_int, C.c_int, C.c_int32, _P, C.c_size_t, C.POINTER(C.c_size_t), _P]),
+    "amb_cog_jpeg_max_size": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int, C.c_int32, C.c_int, C.c_int]),
+    "amb_cog_jpeg_tables": (C.c_int, [C.c_int, C.c_int, _P, C.c_size_t, C.POINTER(C.c_size_t)]),
+    "amb_cog_jpeg_tiles_device": (C.c_int, [_P, _P, C.c_int32, C.c_int32, C.c_size_t, C.c_int, C.c_int32, C.c_int,
+                                            C.c_int, _P, C.c_size_t, C.POINTER(C.c_size_t), _P]),
+    "amb_export_cog_jpeg_tiles": (C.c_int, [_P, C.c_int, C.c_int, C.c_int32, C.c_int, C.c_int, _P, C.c_size_t,
+                                            C.POINTER(C.c_size_t), _P]),
+    "amb_cog_mask_max_size": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),
+    "amb_cog_mask_tiles_device": (C.c_int, [_P, _P, C.c_int32, C.c_int32, C.c_size_t, C.c_int32, _P, C.c_size_t,
+                                            C.POINTER(C.c_size_t), _P]),
+    "amb_export_cog_mask_tiles": (C.c_int, [_P, C.c_int, C.c_int32, _P, C.c_size_t, C.POINTER(C.c_size_t), _P]),
     "amb_get_timings": (C.c_int, [_P, C.POINTER(Timings)]),
     "amb_host_alloc": (C.c_int, [C.POINTER(_P), C.c_size_t]),
     "amb_host_free": (C.c_int, [_P]),

@@ -286,12 +286,19 @@ class GridMap(object):
         from . import io
         io.write_geotiff_strips(path, data, counts, width, height, fmt, rps, gt, epsg, nodata)
 
-    def to_cog(self, path, name, fmt=None, epsg=32632, nodata=None, tile_size=512):
+    def to_cog(self, path, name, fmt=None, epsg=32632, nodata=None, tile_size=512, compress="deflate", quality=75,
+               sampling="420", mask=None):
         """Writes the context's band of layer `name` to `path` as a Cloud-Optimized GeoTIFF: T x T Deflate tiles with
         internal overviews halved until one fits a tile, pyramid, tiles and compression on the device (convention:
         include/aerial_mapper_b200.h, amb_cog_tiles_device; layout: io.write_cog).  Level 0 reads back as to_raster(name,
         fmt) bit for bit.  fmt and the geotransform as to_geotiff.  nodata must agree with the overviews: "nan" (or NaN)
-        for "f32", 0 for "mask8", none for "gray8" and "bgr8".  tile_size: a multiple of 16 in [16, 4096]."""
+        for "f32", 0 for "mask8", none for "gray8" and "bgr8".  tile_size: a multiple of 16 in [16, 4096].
+
+        compress="jpeg": JPEG tiles in YCbCr ("bgr8") or gray ("gray8") at `quality` (1..100) and `sampling` ("420" or
+        "444"), encoded on the device (amb_cog_jpeg_tiles_device), GDAL's COMPRESS=JPEG layout; no nodata.
+        mask: the name of a layer whose "mask8" export (valid where the layer is not NaN, e.g. "observation_index")
+        becomes the file's internal 1-bit mask (amb_cog_mask_tiles_device), for "gray8" and "bgr8" with either
+        compression: unobserved cells read as no-data instead of image content."""
         if not self._resident:
             raise AmbError(_lib.AMB_ERR_INVALID_ARGUMENT, "to_cog exports device-resident layers: call to_device() first")
         if fmt is None:
@@ -300,6 +307,15 @@ class GridMap(object):
                 raise ValueError("to_cog(%r): give fmt='f32', 'gray8', 'bgr8' or 'mask8' for this layer" % (name,))
         if fmt not in _lib.RASTER_FORMAT:
             raise ValueError("to_cog: fmt must be 'f32', 'gray8', 'bgr8' or 'mask8', got %r" % (fmt,))
+        if compress not in ("deflate", "jpeg"):
+            raise ValueError("to_cog: compress must be 'deflate' or 'jpeg', got %r" % (compress,))
+        jpeg = compress == "jpeg"
+        if (jpeg or mask is not None) and fmt not in ("gray8", "bgr8"):
+            raise ValueError("to_cog: %s is for fmt 'gray8' and 'bgr8' only, got %r" % ("JPEG" if jpeg else "mask", fmt))
+        if jpeg and nodata is not None:
+            raise ValueError("to_cog: a JPEG COG takes no nodata (JPEG is lossy): give mask= instead")
+        if mask is not None and mask not in LAYER_ID:
+            raise ValueError("to_cog: mask must be a layer name, got %r" % (mask,))
         from . import io
         io.cog_nodata(fmt, nodata)
         tile = _cog_tile(tile_size)
@@ -307,12 +323,27 @@ class GridMap(object):
         c0, c1 = self._col_range
         width, height = self.geometry.rows, c1 - c0
         ctx = self._ctx
-        data, counts = _cog_call(
-            lambda buf, cap, size, tb: lib().amb_export_cog_tiles(ctx, LAYER_ID[name], f, tile, buf, cap, size, tb),
-            width, height, f, tile, ctx)
+        tables = None
+        if jpeg:
+            q, s = _cog_jpeg_args(quality, sampling)
+            data, counts = _cog_jpeg_call(
+                lambda buf, cap, size, tb: lib().amb_export_cog_jpeg_tiles(ctx, LAYER_ID[name], f, tile, q, s, buf, cap,
+                                                                           size, tb),
+                width, height, f, tile, q, s, ctx)
+            tables = cog_jpeg_tables(fmt, quality)
+        else:
+            data, counts = _cog_call(
+                lambda buf, cap, size, tb: lib().amb_export_cog_tiles(ctx, LAYER_ID[name], f, tile, buf, cap, size, tb),
+                width, height, f, tile, ctx)
+        masks = None
+        if mask is not None:
+            masks = _cog_call(
+                lambda buf, cap, size, tb: lib().amb_export_cog_mask_tiles(ctx, LAYER_ID[mask], tile, buf, cap, size, tb),
+                width, height, _lib.RASTER_MASK8, tile, ctx, cap=lib().amb_cog_mask_max_size(width, height, tile))
         gt = list(self.geotransform())
         gt[3] += c0 * gt[5]        # the band's north edge
-        io.write_cog(path, data, counts, width, height, fmt, tile, gt, epsg, nodata)
+        io.write_cog(path, data, counts, width, height, fmt, tile, gt, epsg, nodata, compress=compress,
+                     jpeg_tables=tables, sampling=sampling, mask=masks)
 
     def timings(self):
         t = _lib.Timings()
@@ -974,10 +1005,11 @@ def _cog_tile(tile_size):
     return int(tile_size)
 
 
-def _cog_call(call, width, height, fmt, tile, ctx):
-    """Runs `call(buffer, capacity, size, tile_bytes)` with a buffer of amb_cog_max_size bytes; returns the tiles in file
-    order (bytes) and their lengths (uint32 array)."""
-    cap = lib().amb_cog_max_size(width, height, fmt, tile)
+def _cog_call(call, width, height, fmt, tile, ctx, cap=None):
+    """Runs `call(buffer, capacity, size, tile_bytes)` with a buffer of `cap` bytes (by default amb_cog_max_size);
+    returns the tiles in file order (bytes) and their lengths (uint32 array)."""
+    if cap is None:
+        cap = lib().amb_cog_max_size(width, height, fmt, tile)
     if cap == 0:
         raise AmbError(_lib.AMB_ERR_UNSUPPORTED, "a %d x %d raster in tiles of %d" % (width, height, tile))
     from . import io
@@ -999,3 +1031,78 @@ def cog_tiles(image, fmt, tile_size=512):
     return _cog_call(
         lambda buf, cap, size, tb: lib().amb_cog_tiles_device(ctx, C.c_void_p(image.data_ptr()), w, h, stride, f, tile,
                                                               buf, cap, size, tb), w, h, f, tile, ctx)
+
+
+# ---- JPEG and mask tiles of a Cloud-Optimized GeoTIFF (amb_cog_jpeg_tiles_device, amb_cog_mask_tiles_device) ------------
+def _cog_jpeg_args(quality, sampling):
+    """Checks quality and sampling (ValueError otherwise); returns their C values."""
+    if sampling not in JPEG_SAMPLING:
+        raise ValueError("JPEG sampling must be '420' or '444', got %r" % (sampling,))
+    if isinstance(quality, bool) or not isinstance(quality, (int, np.integer)) or not 1 <= quality <= 100:
+        raise ValueError("JPEG quality must be an integer in [1, 100], got %r" % (quality,))
+    return int(quality), JPEG_SAMPLING[sampling]
+
+
+def _cog_jpeg_call(call, width, height, fmt, tile, quality, sampling, ctx):
+    """Runs `call(buffer, capacity, size, tile_bytes)`, first with a buffer the size of the raw stacked tiles, again at
+    the size the library reports if the tiles are larger (incompressible content); returns the tiles in file order
+    (bytes) and their lengths (uint32 array)."""
+    if lib().amb_cog_jpeg_max_size(width, height, fmt, tile, quality, sampling) == 0:
+        raise AmbError(_lib.AMB_ERR_UNSUPPORTED, "JPEG tiles of a %d x %d raster in tiles of %d" % (width, height, tile))
+    from . import io
+    n_tiles = sum(-(-w // tile) * -(-h // tile) for w, h in io.cog_layout(width, height, tile))
+    cap = n_tiles * (tile * tile * _lib.RASTER_BPP[fmt] + 64)
+    for _ in range(2):
+        buf = np.empty(cap, np.uint8)
+        counts = np.zeros(n_tiles, np.uint32)
+        size = C.c_size_t(0)
+        st = call(buf.ctypes.data_as(C.c_void_p), cap, C.byref(size), counts.ctypes.data_as(C.c_void_p))
+        if st == _lib.AMB_ERR_SIZE_MISMATCH and size.value > cap:
+            cap = size.value
+            continue
+        check(st, ctx)
+        return buf[:size.value].tobytes(), counts
+    raise AmbError(_lib.AMB_ERR_SIZE_MISMATCH, "JPEG tiles changed size between two encodes of the same raster")
+
+
+def cog_jpeg_tables(fmt, quality=75):
+    """The JPEGTables stream (bytes: SOI, DQT ..., DHT ..., EOI, what cv2.imencode writes) of the JPEG tiles of a "gray8"
+    or "bgr8" raster at `quality`; host only (amb_cog_jpeg_tables)."""
+    if fmt not in ("gray8", "bgr8"):
+        raise ValueError("cog_jpeg_tables: fmt must be 'gray8' or 'bgr8', got %r" % (fmt,))
+    q, _ = _cog_jpeg_args(quality, "420")
+    buf = np.empty(1024, np.uint8)
+    size = C.c_size_t(0)
+    check(lib().amb_cog_jpeg_tables(3 if fmt == "bgr8" else 1, q, buf.ctypes.data_as(C.c_void_p), len(buf),
+                                    C.byref(size)))
+    return buf[:size.value].tobytes()
+
+
+def cog_jpeg_tiles(image, fmt, tile_size=512, quality=75, sampling="420"):
+    """The JPEG tiles of a Cloud-Optimized GeoTIFF of a torch CUDA "gray8" or "bgr8" raster: overview pyramid, tiling and
+    JPEG on its device (convention: include/aerial_mapper_b200.h, amb_cog_jpeg_tiles_device).  Returns (tiles as bytes
+    in file order, uint32 length of each tile, the JPEGTables stream), ready for io.write_cog(..., compress="jpeg").
+    image as for cog_tiles; quality 1..100, sampling "420" or "444" (ignored for gray)."""
+    if fmt not in ("gray8", "bgr8"):
+        raise ValueError("cog_jpeg_tiles: fmt must be 'gray8' or 'bgr8', got %r" % (fmt,))
+    tile = _cog_tile(tile_size)
+    q, s = _cog_jpeg_args(quality, sampling)
+    h, w, f, stride, ctx = _device_raster(image, fmt, "cog_jpeg_tiles")
+    data, counts = _cog_jpeg_call(
+        lambda buf, cap, size, tb: lib().amb_cog_jpeg_tiles_device(ctx, C.c_void_p(image.data_ptr()), w, h, stride, f,
+                                                                   tile, q, s, buf, cap, size, tb), w, h, f, tile, q, s,
+        ctx)
+    return data, counts, cog_jpeg_tables(fmt, q)
+
+
+def cog_mask_tiles(image, tile_size=512):
+    """The 1-bit mask tiles of a Cloud-Optimized GeoTIFF of a torch CUDA uint8 H x W "mask8" raster (non-zero = valid):
+    its MASK8 pyramid, tiled, packed to bits and deflated on its device (convention: include/aerial_mapper_b200.h,
+    amb_cog_mask_tiles_device).  Returns (tiles as bytes in file order, uint32 length of each tile), the `mask` of
+    io.write_cog."""
+    tile = _cog_tile(tile_size)
+    h, w, f, stride, ctx = _device_raster(image, "mask8", "cog_mask_tiles")
+    return _cog_call(
+        lambda buf, cap, size, tb: lib().amb_cog_mask_tiles_device(ctx, C.c_void_p(image.data_ptr()), w, h, stride, tile,
+                                                                   buf, cap, size, tb), w, h, f, tile, ctx,
+        cap=lib().amb_cog_mask_max_size(w, h, tile))

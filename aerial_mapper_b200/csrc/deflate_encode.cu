@@ -84,7 +84,7 @@ __global__ void __launch_bounds__(256)
     const unsigned long long r = i / s.row_bytes, k = i - r * s.row_bytes;
     const unsigned char* row = s.img + r * s.stride;
     unsigned int v = row_byte(s, row, k);
-    if (k >= static_cast<unsigned long long>(step)) v -= row_byte(s, row, k - step);
+    if (s.predict && k >= static_cast<unsigned long long>(step)) v -= row_byte(s, row, k - step);
     out[i] = static_cast<unsigned char>(v);
   }
 }
@@ -758,8 +758,8 @@ size_t align256(size_t v) { return (v + 255) & ~size_t(255); }
 
 }  // namespace
 
-int deflate_params(int32_t w, int32_t h, int format, int32_t rps, DeflateParams* p) {
-  if (w <= 0 || h <= 0 || rps <= 0) return AMB_ERR_INVALID_ARGUMENT;
+int deflate_params(int32_t w, int32_t h, int format, int32_t rps, DeflateParams* p, bool predictor) {
+  if (w <= 0 || h <= 0 || rps <= 0 || (!predictor && format == AMB_RASTER_F32)) return AMB_ERR_INVALID_ARGUMENT;
   DeflateShape& s = p->s;
   switch (format) {
     case AMB_RASTER_F32: s.spp = 1; s.bps = 4; break;
@@ -768,6 +768,7 @@ int deflate_params(int32_t w, int32_t h, int format, int32_t rps, DeflateParams*
     case AMB_RASTER_BGR8: s.spp = 3; s.bps = 1; break;
     default: return AMB_ERR_INVALID_ARGUMENT;
   }
+  s.predict = predictor ? 1 : 0;
   s.img = nullptr;
   s.stride = 0;
   s.w = w;

@@ -12,6 +12,7 @@ struct DeflateShape {
   unsigned long long stride;     // bytes between raster rows
   int32_t w, h;
   int32_t spp, bps;              // samples per pixel, bytes per sample
+  int32_t predict;               // 1: the TIFF predictor of the format; 0: the bytes as they are (a COG's 1-bit masks)
   unsigned long long row_bytes;  // predicted bytes per row = w * spp * bps
   int32_t rps;                   // rows per strip
   int32_t n_strips;
@@ -27,8 +28,9 @@ struct DeflateParams {
   unsigned long long bound;    // the largest file
 };
 
-// AMB_OK, AMB_ERR_INVALID_ARGUMENT or AMB_ERR_UNSUPPORTED (a strip over 4 GiB, which TIFF cannot count)
-int deflate_params(int32_t w, int32_t h, int format, int32_t rps, DeflateParams* p);
+// AMB_OK, AMB_ERR_INVALID_ARGUMENT or AMB_ERR_UNSUPPORTED (a strip over 4 GiB, which TIFF cannot count).  predictor
+// false: no predictor (TIFF Predictor 1), for 8-bit formats only.
+int deflate_params(int32_t w, int32_t h, int format, int32_t rps, DeflateParams* p, bool predictor = true);
 
 // The strips of the w x h raster at d_img (rows row_stride bytes apart), ordered after earlier work on the context's
 // stream; synchronous, with the capacity contract of amb_deflate_strips_device.  Arguments are checked by the caller.

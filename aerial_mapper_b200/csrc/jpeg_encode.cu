@@ -14,6 +14,8 @@
 //            last MCU of a restart interval pads it with 1 bits
 //   stuff    0xFF bytes counted per 4 KB chunk, scan, then a copy that inserts 0x00 after every 0xFF and places
 //            RST(n mod 8) in front of restart interval n >= 1
+// The JPEG tiles of a Cloud-Optimized GeoTIFF (jpeg_encode.h) replace the last copy by a split: every restart interval,
+// stuffed, becomes a stream of its own with a tile header in front and EOI behind, and no RST markers.
 // Coefficients are recomputed by the pack step rather than stored: the scratch stays at ~0.08 (4:2:0) / 0.22 (4:4:4)
 // byte per pixel plus the compressed stream twice, at any image size.
 // Integer widths: every DCT intermediate fits int32 (|pass-1 output| <= 5793 for level-shifted 8-bit samples; the
@@ -21,7 +23,7 @@
 #include <algorithm>
 #include <cstring>
 
-#include "amb_context.h"
+#include "jpeg_encode.h"
 
 namespace amb {
 namespace {
@@ -417,20 +419,72 @@ __global__ void __launch_bounds__(kStuffThreads)
   }
 }
 
-// ---- host side -------------------------------------------------------------------------------------------------------
-struct JpegParams {
-  int32_t w, h;
-  int channels, quality, sampling;
-  int32_t interval;
-  int bpm, mcus_x, mcus_y, kind;
-  unsigned long long n_mcu, n_seg;
+// The constant header of every tile stream of jpeg_split_kernel: SOI, SOF0, SOS
+struct TileHead {
+  unsigned char b[48];
+  int32_t len;
 };
 
-// AMB_OK, AMB_ERR_INVALID_ARGUMENT (malformed) or AMB_ERR_UNSUPPORTED (outside the supported parameter set)
-int jpeg_params(int32_t w, int32_t h, int channels, int quality, int sampling, int32_t interval, JpegParams* p) {
-  if (w <= 0 || h <= 0) return AMB_ERR_INVALID_ARGUMENT;
-  if (w > 65535 || h > 65535 || (channels != 1 && channels != 3) || quality < 1 || quality > 100 ||
-      (sampling != AMB_JPEG_420 && sampling != AMB_JPEG_444) || interval < 0 || interval > 65535)
+// split, 2: byte i of interval sg goes to i + (0xFF bytes before it) + sg * (head.len + 2) + head.len, so that every
+// interval becomes a stream of its own: the header in front, EOI behind, no RST marker.  start[sg]: where its stream
+// begins (every interval holds at least one byte, so exactly one thread meets its first byte).
+__global__ void __launch_bounds__(kStuffThreads)
+    jpeg_split_kernel(const uint32_t* __restrict__ words, unsigned long long n_bytes,
+                      const unsigned long long* __restrict__ ff_off, const unsigned long long* __restrict__ seg_off,
+                      unsigned long long n_seg, const TileHead head, unsigned char* __restrict__ out,
+                      unsigned long long* __restrict__ start) {
+  const unsigned long long i0 = static_cast<unsigned long long>(blockIdx.x) * kStuffChunk + threadIdx.x * kStuffBytes;
+  unsigned long long c = 0;
+  for (int k = 0; k < kStuffBytes; ++k)
+    if (i0 + k < n_bytes && stream_byte(words, i0 + k) == 0xffu) ++c;
+  unsigned long long total;
+  unsigned long long ff = ff_off[blockIdx.x] + block_exclusive<kStuffThreads>(c, &total);
+  if (i0 >= n_bytes) return;
+  unsigned long long lo = 0, hi = n_seg - 1;  // the last interval starting at or before i0
+  while (lo < hi) {
+    const unsigned long long mid = (lo + hi + 1) >> 1;
+    if (seg_off[mid] <= i0)
+      lo = mid;
+    else
+      hi = mid - 1;
+  }
+  unsigned long long sg = lo;
+  const unsigned long long gap = static_cast<unsigned long long>(head.len) + 2;
+  for (int k = 0; k < kStuffBytes && i0 + k < n_bytes; ++k) {
+    const unsigned long long i = i0 + k;
+    while (sg + 1 < n_seg && seg_off[sg + 1] <= i) ++sg;
+    const unsigned long long p = i + ff + sg * gap + head.len;
+    if (seg_off[sg] == i) {
+      for (int j = 0; j < head.len; ++j) out[p - head.len + j] = head.b[j];
+      start[sg] = p - head.len;
+    }
+    const unsigned int b = stream_byte(words, i);
+    out[p] = static_cast<unsigned char>(b);
+    unsigned long long e = p + 1;
+    if (b == 0xffu) {
+      out[e++] = 0;
+      ++ff;
+    }
+    if (i + 1 == (sg + 1 < n_seg ? seg_off[sg + 1] : n_bytes)) {  // the interval's last byte: EOI
+      out[e] = 0xff;
+      out[e + 1] = 0xd9;
+    }
+  }
+}
+
+// the length of every stream of jpeg_split_kernel, `total` bytes in all
+__global__ void jpeg_tile_bytes_kernel(const unsigned long long* __restrict__ start, unsigned long long n_seg,
+                                       unsigned long long total, uint32_t* __restrict__ len) {
+  const unsigned long long k = static_cast<unsigned long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (k < n_seg) len[k] = static_cast<uint32_t>((k + 1 < n_seg ? start[k + 1] : total) - start[k]);
+}
+
+// ---- host side -------------------------------------------------------------------------------------------------------
+// The image's MCU grid, without the 65535 limits of the file format: AMB_OK or AMB_ERR_UNSUPPORTED (channels, quality,
+// sampling, a negative interval); w, h > 0 are the caller's to check
+int jpeg_shape(int32_t w, int32_t h, int channels, int quality, int sampling, int32_t interval, JpegParams* p) {
+  if ((channels != 1 && channels != 3) || quality < 1 || quality > 100 ||
+      (sampling != AMB_JPEG_420 && sampling != AMB_JPEG_444) || interval < 0)
     return AMB_ERR_UNSUPPORTED;
   p->w = w;
   p->h = h;
@@ -446,6 +500,13 @@ int jpeg_params(int32_t w, int32_t h, int channels, int quality, int sampling, i
   p->n_mcu = static_cast<unsigned long long>(p->mcus_x) * static_cast<unsigned long long>(p->mcus_y);
   p->n_seg = interval ? (p->n_mcu + interval - 1) / interval : 1ull;
   return AMB_OK;
+}
+
+// AMB_OK, AMB_ERR_INVALID_ARGUMENT (malformed) or AMB_ERR_UNSUPPORTED (outside the supported parameter set)
+int jpeg_params(int32_t w, int32_t h, int channels, int quality, int sampling, int32_t interval, JpegParams* p) {
+  if (w <= 0 || h <= 0) return AMB_ERR_INVALID_ARGUMENT;
+  if (w > 65535 || h > 65535 || interval > 65535) return AMB_ERR_UNSUPPORTED;
+  return jpeg_shape(w, h, channels, quality, sampling, interval, p);
 }
 
 // jcparam.c jpeg_quality_scaling + jpeg_add_quant_table(force_baseline)
@@ -492,12 +553,8 @@ void put_dht(std::vector<unsigned char>& h, int cls_id, const uint8_t* bits, con
   h.insert(h.end(), vals, vals + n);
 }
 
-// SOI, APP0 JFIF 1.01, DQT per table, SOF0, DHT DC0 AC0 [DC1 AC1], DRI if restarts, SOS — libjpeg's order
-std::vector<unsigned char> jpeg_header(const JpegParams& p) {
-  std::vector<unsigned char> h = {0xff, 0xd8, 0xff, 0xe0, 0x00, 0x10, 'J', 'F', 'I', 'F', 0x00,
-                                  0x01, 0x01, 0x00, 0x00, 0x01, 0x00, 0x01, 0x00, 0x00};
-  const int nc = p.channels;
-  for (int c = 0; c < (nc == 3 ? 2 : 1); ++c) {
+void put_dqt(std::vector<unsigned char>& h, const JpegParams& p) {  // one DQT per table
+  for (int c = 0; c < (p.channels == 3 ? 2 : 1); ++c) {
     uint8_t q[64];
     quant_table(c ? kChromaQuant : kLumQuant, p.quality, q);
     h.push_back(0xff);
@@ -506,6 +563,10 @@ std::vector<unsigned char> jpeg_header(const JpegParams& p) {
     h.push_back(static_cast<unsigned char>(c));
     for (int k = 0; k < 64; ++k) h.push_back(q[kZigzag[k]]);
   }
+}
+
+void put_sof(std::vector<unsigned char>& h, const JpegParams& p) {
+  const int nc = p.channels;
   h.push_back(0xff);
   h.push_back(0xc0);
   put16(h, 8 + 3 * nc);
@@ -518,18 +579,19 @@ std::vector<unsigned char> jpeg_header(const JpegParams& p) {
     h.push_back(c == 0 && p.kind == 2 ? 0x22 : 0x11);
     h.push_back(c == 0 ? 0 : 1);
   }
+}
+
+void put_dhts(std::vector<unsigned char>& h, const JpegParams& p) {  // DC0 AC0 [DC1 AC1]
   put_dht(h, 0x00, kDcLumBits, kDcVals);
   put_dht(h, 0x10, kAcLumBits, kAcLumVals);
-  if (nc == 3) {
+  if (p.channels == 3) {
     put_dht(h, 0x01, kDcChromaBits, kDcVals);
     put_dht(h, 0x11, kAcChromaBits, kAcChromaVals);
   }
-  if (p.interval) {
-    h.push_back(0xff);
-    h.push_back(0xdd);
-    put16(h, 4);
-    put16(h, p.interval);
-  }
+}
+
+void put_sos(std::vector<unsigned char>& h, const JpegParams& p) {
+  const int nc = p.channels;
   h.push_back(0xff);
   h.push_back(0xda);
   put16(h, 6 + 2 * nc);
@@ -541,6 +603,22 @@ std::vector<unsigned char> jpeg_header(const JpegParams& p) {
   h.push_back(0);
   h.push_back(63);
   h.push_back(0);
+}
+
+// SOI, APP0 JFIF 1.01, DQT per table, SOF0, DHT DC0 AC0 [DC1 AC1], DRI if restarts, SOS — libjpeg's order
+std::vector<unsigned char> jpeg_header(const JpegParams& p) {
+  std::vector<unsigned char> h = {0xff, 0xd8, 0xff, 0xe0, 0x00, 0x10, 'J', 'F', 'I', 'F', 0x00,
+                                  0x01, 0x01, 0x00, 0x00, 0x01, 0x00, 0x01, 0x00, 0x00};
+  put_dqt(h, p);
+  put_sof(h, p);
+  put_dhts(h, p);
+  if (p.interval) {
+    h.push_back(0xff);
+    h.push_back(0xdd);
+    put16(h, 4);
+    put16(h, p.interval);
+  }
+  put_sos(h, p);
   return h;
 }
 
@@ -548,8 +626,16 @@ unsigned int grid_of(unsigned long long n, int threads) {
   return static_cast<unsigned int>((n + threads - 1) / threads);
 }
 
-int jpeg_encode(amb_ctx* ctx, const unsigned char* d_img, size_t row_stride, const JpegParams& p, void* host_out,
-                size_t capacity, size_t* size) {
+// The entropy-coded stream before byte stuffing, on the device: what the stuff and split steps read
+struct JpegScan {
+  const unsigned long long* seg_off;  // byte offset of every interval, n_seg + 1 entries
+  const uint32_t* words;              // the stream
+  const unsigned long long* ff_off;   // 0xFF bytes before every chunk of kStuffChunk bytes
+  unsigned long long n_bytes, n_chunks, n_ff;
+};
+
+// measure, length, segments, pack and the 0xFF count of the image at d_img
+int jpeg_scan(amb_ctx* ctx, const unsigned char* d_img, size_t row_stride, const JpegParams& p, JpegScan* r) {
   JpegShape s;
   s.img = d_img;
   s.stride = row_stride;
@@ -565,7 +651,6 @@ int jpeg_encode(amb_ctx* ctx, const unsigned char* d_img, size_t row_stride, con
   s.c_rows = (p.h + 1) / 2;
   JpegTables t;
   jpeg_tables(p, &t);
-  const std::vector<unsigned char> header = jpeg_header(p);
   cudaStream_t st = ctx->stream;
 
   // per MCU: DC values, bit lengths -> offsets (+ total), and the scan spine; per interval: byte lengths -> offsets
@@ -605,14 +690,25 @@ int jpeg_encode(amb_ctx* ctx, const unsigned char* d_img, size_t row_stride, con
   unsigned long long n_ff = 0;
   rc = read_u64(ctx, ff_off + n_chunks, &n_ff);
   if (rc != AMB_OK) return rc;
+  *r = JpegScan{seg_off, words, ff_off, n_bytes, n_chunks, n_ff};
+  return AMB_OK;
+}
 
-  const size_t data = static_cast<size_t>(n_bytes + n_ff + 2 * (ns - 1));
+int jpeg_encode(amb_ctx* ctx, const unsigned char* d_img, size_t row_stride, const JpegParams& p, void* host_out,
+                size_t capacity, size_t* size) {
+  JpegScan r;
+  int rc = jpeg_scan(ctx, d_img, row_stride, p, &r);
+  if (rc != AMB_OK) return rc;
+  const std::vector<unsigned char> header = jpeg_header(p);
+  const unsigned long long ns = p.n_seg;
+  const size_t data = static_cast<size_t>(r.n_bytes + r.n_ff + 2 * (ns - 1));
   const size_t total = header.size() + data + 2;
   *size = total;
   if (capacity < total) return AMB_ERR_SIZE_MISMATCH;
+  cudaStream_t st = ctx->stream;
   AMB_CUDA(ctx, ctx->jpeg_out.reserve(data));
-  jpeg_stuff_kernel<<<static_cast<unsigned int>(n_chunks), kStuffThreads, 0, st>>>(words, n_bytes, ff_off, seg_off, ns,
-                                                                                   ctx->jpeg_out.as<unsigned char>());
+  jpeg_stuff_kernel<<<static_cast<unsigned int>(r.n_chunks), kStuffThreads, 0, st>>>(
+      r.words, r.n_bytes, r.ff_off, r.seg_off, ns, ctx->jpeg_out.as<unsigned char>());
   AMB_CUDA(ctx, cudaGetLastError());
   unsigned char* out = static_cast<unsigned char*>(host_out);
   rc = staged_d2h(ctx, out + header.size(), ctx->jpeg_out.ptr, data, st);
@@ -624,6 +720,69 @@ int jpeg_encode(amb_ctx* ctx, const unsigned char* d_img, size_t row_stride, con
 }
 
 }  // namespace
+
+int jpeg_tile_params(int32_t tile, long long n_tiles, int channels, int quality, int sampling, JpegParams* p) {
+  if (tile <= 0 || tile % 16 != 0 || n_tiles <= 0 || n_tiles * tile > 0x7fffffffll) return AMB_ERR_UNSUPPORTED;
+  const int st = jpeg_shape(tile, static_cast<int32_t>(n_tiles * tile), channels, quality, sampling, 0, p);
+  if (st != AMB_OK) return st;
+  const int32_t side = tile / (p->kind == 2 ? 16 : 8);  // MCUs along a tile side
+  p->interval = side * side;
+  p->n_seg = static_cast<unsigned long long>(n_tiles);
+  return AMB_OK;
+}
+
+unsigned long long jpeg_tiles_bound(const JpegParams& p) {
+  // as amb_jpeg_max_size: every interval adds < 1 byte of padding, stuffing at most doubles the bytes; per tile the
+  // header and EOI in place of the file's header and RST markers
+  const unsigned long long head = 2 + 10 + 3 * p.channels + 8 + 2 * p.channels;  // SOI, SOF0, SOS
+  const unsigned long long bytes = (p.n_mcu * p.bpm * (22 + 63 * 26) + 7) / 8 + p.n_seg;
+  return 2 * bytes + (head + 2) * p.n_seg;
+}
+
+std::vector<unsigned char> jpeg_tables_stream(int channels, int quality) {
+  JpegParams p{};
+  p.channels = channels;
+  p.quality = quality;
+  std::vector<unsigned char> h = {0xff, 0xd8};
+  put_dqt(h, p);
+  put_dhts(h, p);
+  h.push_back(0xff);
+  h.push_back(0xd9);
+  return h;
+}
+
+int jpeg_tiles_encode(amb_ctx* ctx, const unsigned char* d_img, size_t row_stride, const JpegParams& p,
+                      void* host_out, size_t capacity, size_t* size, uint32_t* tile_bytes) {
+  JpegScan r;
+  int rc = jpeg_scan(ctx, d_img, row_stride, p, &r);
+  if (rc != AMB_OK) return rc;
+  JpegParams tp = p;  // the header of one tile: SOI, SOF0 (tile x tile), SOS
+  tp.h = p.w;
+  std::vector<unsigned char> h = {0xff, 0xd8};
+  put_sof(h, tp);
+  put_sos(h, tp);
+  TileHead head;
+  std::memcpy(head.b, h.data(), h.size());
+  head.len = static_cast<int32_t>(h.size());
+  const unsigned long long ns = p.n_seg;
+  const size_t total = static_cast<size_t>(r.n_bytes + r.n_ff + ns * (h.size() + 2));
+  *size = total;
+  if (capacity < total) return AMB_ERR_SIZE_MISMATCH;
+  cudaStream_t st = ctx->stream;
+  const size_t data_bytes = (total + 255) & ~size_t(255);
+  AMB_CUDA(ctx, ctx->jpeg_out.reserve(data_bytes + ns * 8 + ns * 4));
+  unsigned char* out = ctx->jpeg_out.as<unsigned char>();
+  unsigned long long* start = reinterpret_cast<unsigned long long*>(out + data_bytes);
+  uint32_t* lens = reinterpret_cast<uint32_t*>(start + ns);
+  jpeg_split_kernel<<<static_cast<unsigned int>(r.n_chunks), kStuffThreads, 0, st>>>(r.words, r.n_bytes, r.ff_off,
+                                                                                     r.seg_off, ns, head, out, start);
+  jpeg_tile_bytes_kernel<<<grid_of(ns, 256), 256, 0, st>>>(start, ns, total, lens);
+  AMB_CUDA(ctx, cudaGetLastError());
+  rc = staged_d2h(ctx, host_out, out, total, st);
+  if (rc != AMB_OK) return rc;
+  return staged_d2h(ctx, tile_bytes, lens, static_cast<size_t>(ns) * 4, st);
+}
+
 }  // namespace amb
 
 using namespace amb;

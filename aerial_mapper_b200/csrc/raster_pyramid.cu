@@ -8,10 +8,14 @@
 //           outside the level zero.  All tiles of all levels go into one buffer, smallest level first,
 //           each level's tiles row-major, so the buffer is a raster T pixels wide and n_tiles * T rows high.
 //   deflate that raster compressed by deflate_encode (deflate_encode.cu) in strips of T rows: strip k is tile k.
+// The JPEG tiles (amb_cog_jpeg_tiles_device) encode the stacked raster instead as one JPEG image with a restart interval
+// per tile, split into one abbreviated stream per tile (jpeg_encode.cu).  The 1-bit mask tiles (amb_cog_mask_tiles_device)
+// pack the stacked MASK8 tiles to bits (mask_pack_kernel) and deflate them without a predictor.
 // One-dimensional grids with grid-stride loops over rows and tiles; offsets are 64-bit.
 #include <algorithm>
 
 #include "deflate_encode.h"
+#include "jpeg_encode.h"
 
 namespace amb {
 namespace {
@@ -169,6 +173,22 @@ __global__ void __launch_bounds__(256)
   }
 }
 
+// ---- mask ------------------------------------------------------------------------------------------------------------------
+// The stacked MASK8 tiles (n pieces of 16 bytes) at 1 bit per pixel, most significant bit first, 1 where the byte is not
+// 0: piece i becomes bytes 2i and 2i + 1.  A tile row is T / 16 whole pieces (16 | T), so rows of T / 8 bytes.
+__global__ void __launch_bounds__(256)
+    mask_pack_kernel(const uint4* __restrict__ src, unsigned long long n, uint16_t* __restrict__ dst) {
+  for (unsigned long long i = static_cast<unsigned long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n;
+       i += static_cast<unsigned long long>(gridDim.x) * blockDim.x) {
+    const uint4 v = __ldg(src + i);
+    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+    uint32_t bits = 0;  // pixel q at bit 15 - q
+#pragma unroll
+    for (int q = 0; q < 16; ++q) bits |= (((w[q >> 2] >> (8 * (q & 3))) & 0xffu) != 0u ? 1u : 0u) << (15 - q);
+    dst[i] = static_cast<uint16_t>((bits >> 8) | ((bits & 0xffu) << 8));  // little-endian: pixels 0..7 in the first byte
+  }
+}
+
 // ---- host side ------------------------------------------------------------------------------------------------------------
 struct CogPlan {
   int32_t n_levels;
@@ -180,6 +200,7 @@ struct CogPlan {
   long long n_tiles;
   int32_t tile, bpp;
   DeflateParams deflate;             // the stacked tiles: tile wide, n_tiles * tile high, strips of tile rows
+  JpegParams jpeg;                   // ... or one JPEG image with a restart interval per tile
 };
 
 // The levels alone: AMB_OK or AMB_ERR_INVALID_ARGUMENT
@@ -197,9 +218,9 @@ int cog_levels(int32_t w, int32_t h, int32_t tile, CogPlan* p) {
   return AMB_OK;
 }
 
-// AMB_OK, AMB_ERR_INVALID_ARGUMENT or AMB_ERR_UNSUPPORTED (more tile rows than an int32 counts, or what deflate_params
-// cannot take)
-int cog_plan(int32_t w, int32_t h, int format, int32_t tile, CogPlan* p) {
+// The levels, their tiles and the scratch layout: AMB_OK, AMB_ERR_INVALID_ARGUMENT or AMB_ERR_UNSUPPORTED (more tile
+// rows than an int32 counts)
+int cog_grid(int32_t w, int32_t h, int format, int32_t tile, CogPlan* p) {
   int st = cog_levels(w, h, tile, p);
   if (st != AMB_OK) return st;
   if (format < AMB_RASTER_F32 || format > AMB_RASTER_MASK8) return AMB_ERR_INVALID_ARGUMENT;
@@ -221,7 +242,31 @@ int cog_plan(int32_t w, int32_t h, int format, int32_t tile, CogPlan* p) {
     at += (p->level_pitch[k] * p->h[k] + 255) & ~255ull;
   }
   p->level_bytes = at;
-  return deflate_params(tile, static_cast<int32_t>(n * tile), format, tile, &p->deflate);
+  return AMB_OK;
+}
+
+// AMB_OK, AMB_ERR_INVALID_ARGUMENT or AMB_ERR_UNSUPPORTED (more tile rows than an int32 counts, or what deflate_params
+// cannot take)
+int cog_plan(int32_t w, int32_t h, int format, int32_t tile, CogPlan* p) {
+  const int st = cog_grid(w, h, format, tile, p);
+  if (st != AMB_OK) return st;
+  return deflate_params(tile, static_cast<int32_t>(p->n_tiles * tile), format, tile, &p->deflate);
+}
+
+// JPEG tiles of a GRAY8 or BGR8 raster: AMB_OK, AMB_ERR_INVALID_ARGUMENT (format, sizes, tile side) or
+// AMB_ERR_UNSUPPORTED (quality, sampling, too many tile rows)
+int cog_plan_jpeg(int32_t w, int32_t h, int format, int32_t tile, int quality, int sampling, CogPlan* p) {
+  if (format != AMB_RASTER_GRAY8 && format != AMB_RASTER_BGR8) return AMB_ERR_INVALID_ARGUMENT;
+  const int st = cog_grid(w, h, format, tile, p);
+  if (st != AMB_OK) return st;
+  return jpeg_tile_params(tile, p->n_tiles, format == AMB_RASTER_BGR8 ? 3 : 1, quality, sampling, &p->jpeg);
+}
+
+// 1-bit mask tiles of a MASK8 raster: the packed tiles T / 8 bytes wide, deflated without a predictor
+int cog_plan_mask(int32_t w, int32_t h, int32_t tile, CogPlan* p) {
+  const int st = cog_grid(w, h, AMB_RASTER_MASK8, tile, p);
+  if (st != AMB_OK) return st;
+  return deflate_params(tile / 8, static_cast<int32_t>(p->n_tiles * tile), AMB_RASTER_MASK8, tile, &p->deflate, false);
 }
 
 template <int FMT>
@@ -234,13 +279,14 @@ void launch_reduce(const unsigned char* src, unsigned long long src_stride, int3
   pyramid_reduce_kernel<FMT><<<grid, threads, 0, st>>>(src, src_stride, sw, sh, dst, dst_stride, dw, dh);
 }
 
-int cog_encode(amb_ctx* ctx, const unsigned char* d_img, size_t row_stride, int format, const CogPlan& p,
-               void* host_out, size_t capacity, size_t* size, uint32_t* tile_bytes) {
+// The pyramid of the raster at d_img and its stacked tiles in ctx->cog_tiles (followed by `extra` bytes of scratch)
+int cog_stack(amb_ctx* ctx, const unsigned char* d_img, size_t row_stride, int format, const CogPlan& p,
+              size_t extra) {
   cudaStream_t st = ctx->stream;
   const int T = p.tile;
   const unsigned long long tile_row = static_cast<unsigned long long>(T) * p.bpp;
   AMB_CUDA(ctx, ctx->cog_levels.reserve(std::max<unsigned long long>(p.level_bytes, 1)));
-  AMB_CUDA(ctx, ctx->cog_tiles.reserve(static_cast<size_t>(p.n_tiles) * T * tile_row));
+  AMB_CUDA(ctx, ctx->cog_tiles.reserve(static_cast<size_t>(p.n_tiles) * T * tile_row + extra));
   unsigned char* levels = ctx->cog_levels.as<unsigned char>();
   uint4* tiles = ctx->cog_tiles.as<uint4>();
   const int cap = ctx->num_sms * 16;  // grid-stride launches: blocks per kernel
@@ -272,8 +318,37 @@ int cog_encode(amb_ctx* ctx, const unsigned char* d_img, size_t row_stride, int 
         p.tiles_x[k], n, tiles + p.first_tile[k] * T * (tile_row / 16));
   }
   AMB_CUDA(ctx, cudaGetLastError());
-  return deflate_encode(ctx, reinterpret_cast<const unsigned char*>(tiles), static_cast<size_t>(tile_row), p.deflate,
+  return AMB_OK;
+}
+
+int cog_encode(amb_ctx* ctx, const unsigned char* d_img, size_t row_stride, int format, const CogPlan& p,
+               void* host_out, size_t capacity, size_t* size, uint32_t* tile_bytes) {
+  const int rc = cog_stack(ctx, d_img, row_stride, format, p, 0);
+  if (rc != AMB_OK) return rc;
+  return deflate_encode(ctx, ctx->cog_tiles.as<unsigned char>(), static_cast<size_t>(p.tile) * p.bpp, p.deflate,
                         host_out, capacity, size, tile_bytes);
+}
+
+int cog_encode_jpeg(amb_ctx* ctx, const unsigned char* d_img, size_t row_stride, int format, const CogPlan& p,
+                    void* host_out, size_t capacity, size_t* size, uint32_t* tile_bytes) {
+  const int rc = cog_stack(ctx, d_img, row_stride, format, p, 0);
+  if (rc != AMB_OK) return rc;
+  return jpeg_tiles_encode(ctx, ctx->cog_tiles.as<unsigned char>(), static_cast<size_t>(p.tile) * p.bpp, p.jpeg,
+                           host_out, capacity, size, tile_bytes);
+}
+
+int cog_encode_mask(amb_ctx* ctx, const unsigned char* d_img, size_t row_stride, const CogPlan& p, void* host_out,
+                    size_t capacity, size_t* size, uint32_t* tile_bytes) {
+  const size_t stacked = static_cast<size_t>(p.n_tiles) * p.tile * p.tile;  // MASK8 bytes; the packed bits follow
+  const int rc = cog_stack(ctx, d_img, row_stride, AMB_RASTER_MASK8, p, stacked / 8);
+  if (rc != AMB_OK) return rc;
+  const unsigned long long pieces = stacked / 16;
+  unsigned char* packed = ctx->cog_tiles.as<unsigned char>() + stacked;
+  const int grid = static_cast<int>(std::min<unsigned long long>((pieces + 255) / 256, ctx->num_sms * 16ull));
+  mask_pack_kernel<<<grid, 256, 0, ctx->stream>>>(ctx->cog_tiles.as<uint4>(), pieces,
+                                                  reinterpret_cast<uint16_t*>(packed));
+  AMB_CUDA(ctx, cudaGetLastError());
+  return deflate_encode(ctx, packed, static_cast<size_t>(p.tile / 8), p.deflate, host_out, capacity, size, tile_bytes);
 }
 
 }  // namespace
@@ -327,6 +402,82 @@ int amb_export_cog_tiles(amb_ctx* ctx, int layer, int format, int32_t tile, void
   const int rc = amb_export_raster_device(ctx, layer, format, ctx->raster_band.ptr);
   if (rc != AMB_OK) return rc;
   return cog_encode(ctx, ctx->raster_band.as<unsigned char>(), stride, format, p, host_out, capacity, size, tile_bytes);
+}
+
+size_t amb_cog_jpeg_max_size(int32_t width, int32_t height, int format, int32_t tile, int quality, int sampling) {
+  CogPlan p;
+  if (cog_plan_jpeg(width, height, format, tile, quality, sampling, &p) != AMB_OK) return 0;
+  return static_cast<size_t>(jpeg_tiles_bound(p.jpeg));
+}
+
+int amb_cog_jpeg_tables(int channels, int quality, void* out, size_t capacity, size_t* size) {
+  if (!out || !size) return AMB_ERR_INVALID_ARGUMENT;
+  if ((channels != 1 && channels != 3) || quality < 1 || quality > 100) return AMB_ERR_UNSUPPORTED;
+  const std::vector<unsigned char> t = jpeg_tables_stream(channels, quality);
+  *size = t.size();
+  if (capacity < t.size()) return AMB_ERR_SIZE_MISMATCH;
+  std::copy(t.begin(), t.end(), static_cast<unsigned char*>(out));
+  return AMB_OK;
+}
+
+int amb_cog_jpeg_tiles_device(amb_ctx* ctx, const void* d_image, int32_t width, int32_t height, size_t row_stride,
+                              int format, int32_t tile, int quality, int sampling, void* host_out, size_t capacity,
+                              size_t* size, uint32_t* tile_bytes) {
+  if (!ctx || !d_image || !host_out || !size || !tile_bytes) return AMB_ERR_INVALID_ARGUMENT;
+  CogPlan p;
+  const int st = cog_plan_jpeg(width, height, format, tile, quality, sampling, &p);
+  if (st != AMB_OK) return st;
+  if (row_stride < static_cast<size_t>(width) * p.bpp) return AMB_ERR_INVALID_ARGUMENT;
+  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
+  return cog_encode_jpeg(ctx, static_cast<const unsigned char*>(d_image), row_stride, format, p, host_out, capacity,
+                         size, tile_bytes);
+}
+
+int amb_export_cog_jpeg_tiles(amb_ctx* ctx, int layer, int format, int32_t tile, int quality, int sampling,
+                              void* host_out, size_t capacity, size_t* size, uint32_t* tile_bytes) {
+  if (!ctx || !host_out || !size || !tile_bytes || layer < 0 || layer >= AMB_NUM_LAYERS) return AMB_ERR_INVALID_ARGUMENT;
+  CogPlan p;
+  const int st = cog_plan_jpeg(ctx->geom.rows, ctx->col_end - ctx->col_begin, format, tile, quality, sampling, &p);
+  if (st != AMB_OK) return st;
+  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
+  const size_t stride = static_cast<size_t>(ctx->geom.rows) * p.bpp;
+  AMB_CUDA(ctx, ctx->raster_band.reserve(stride * static_cast<size_t>(ctx->col_end - ctx->col_begin)));
+  const int rc = amb_export_raster_device(ctx, layer, format, ctx->raster_band.ptr);
+  if (rc != AMB_OK) return rc;
+  return cog_encode_jpeg(ctx, ctx->raster_band.as<unsigned char>(), stride, format, p, host_out, capacity, size,
+                         tile_bytes);
+}
+
+size_t amb_cog_mask_max_size(int32_t width, int32_t height, int32_t tile) {
+  CogPlan p;
+  if (cog_plan_mask(width, height, tile, &p) != AMB_OK) return 0;
+  return static_cast<size_t>(p.deflate.bound);
+}
+
+int amb_cog_mask_tiles_device(amb_ctx* ctx, const void* d_mask, int32_t width, int32_t height, size_t row_stride,
+                              int32_t tile, void* host_out, size_t capacity, size_t* size, uint32_t* tile_bytes) {
+  if (!ctx || !d_mask || !host_out || !size || !tile_bytes) return AMB_ERR_INVALID_ARGUMENT;
+  CogPlan p;
+  const int st = cog_plan_mask(width, height, tile, &p);
+  if (st != AMB_OK) return st;
+  if (row_stride < static_cast<size_t>(width)) return AMB_ERR_INVALID_ARGUMENT;
+  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
+  return cog_encode_mask(ctx, static_cast<const unsigned char*>(d_mask), row_stride, p, host_out, capacity, size,
+                         tile_bytes);
+}
+
+int amb_export_cog_mask_tiles(amb_ctx* ctx, int layer, int32_t tile, void* host_out, size_t capacity, size_t* size,
+                              uint32_t* tile_bytes) {
+  if (!ctx || !host_out || !size || !tile_bytes || layer < 0 || layer >= AMB_NUM_LAYERS) return AMB_ERR_INVALID_ARGUMENT;
+  CogPlan p;
+  const int st = cog_plan_mask(ctx->geom.rows, ctx->col_end - ctx->col_begin, tile, &p);
+  if (st != AMB_OK) return st;
+  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
+  const size_t stride = static_cast<size_t>(ctx->geom.rows);
+  AMB_CUDA(ctx, ctx->raster_band.reserve(stride * static_cast<size_t>(ctx->col_end - ctx->col_begin)));
+  const int rc = amb_export_raster_device(ctx, layer, AMB_RASTER_MASK8, ctx->raster_band.ptr);
+  if (rc != AMB_OK) return rc;
+  return cog_encode_mask(ctx, ctx->raster_band.as<unsigned char>(), stride, p, host_out, capacity, size, tile_bytes);
 }
 
 }  // extern "C"

@@ -170,8 +170,8 @@ def load_camera_rig_from_file(filename_ncameras_yaml, camera_index=0):
 
 
 # ---- GeoTIFF (baseline TIFF 6.0 + GeoTIFF 1.0 tags), little-endian, uncompressed or Deflate strips ----
-_SHORT, _ASCII, _LONG, _DOUBLE = 3, 2, 4, 12
-_TYPE_FMT = {_SHORT: "H", _LONG: "I", _DOUBLE: "d"}
+_SHORT, _ASCII, _LONG, _RATIONAL, _UNDEFINED, _DOUBLE = 3, 2, 4, 5, 7, 12
+_TYPE_FMT = {_SHORT: "H", _LONG: "I", _RATIONAL: "I", _DOUBLE: "d"}
 _STRIP_BYTES = 1 << 20
 
 
@@ -196,14 +196,20 @@ def _north_up(geotransform):
     return gt
 
 
-def _image_tags(width, height, bands, bits, predictor, layout, geo=None, subfile=None):
+def _image_tags(width, height, bands, bits, predictor, layout, geo=None, subfile=None, compression=None,
+                photometric=None, extra=()):
     """The tags of one image's IFD in ascending order: `layout` holds its strip or tile tags; predictor None for
     uncompressed data, else Compression 8 (Deflate) with that Predictor; geo (geotransform, epsg, nodata) adds the
-    georeferencing; subfile, if given, NewSubfileType (0 full resolution, 1 reduced)."""
+    georeferencing; subfile, if given, NewSubfileType (0 full resolution, 1 reduced, 4 / 5 their masks).  compression
+    and photometric, if given, replace those the predictor and the bands imply (JPEG, YCbCr, masks); extra: more tags."""
+    if compression is None:
+        compression = 1 if predictor is None else 8
+    if photometric is None:
+        photometric = 2 if bands == 3 else 1
     tags = [(256, _LONG, [width]), (257, _LONG, [height]), (258, _SHORT, [bits] * bands),
-            (259, _SHORT, [1 if predictor is None else 8]), (262, _SHORT, [2 if bands == 3 else 1]),
+            (259, _SHORT, [compression]), (262, _SHORT, [photometric]),
             (277, _SHORT, [bands]), (284, _SHORT, [1]), (339, _SHORT, [3 if bits == 32 else 1] * bands)]
-    tags += list(layout)
+    tags += list(layout) + list(extra)
     if subfile is not None:
         tags.append((254, _LONG, [subfile]))
     if predictor is not None:
@@ -223,7 +229,14 @@ def _image_tags(width, height, bands, bits, predictor, layout, geo=None, subfile
 
 
 def _payload(typ, vals):
-    return bytes(vals) if typ == _ASCII else struct.pack("<%d%s" % (len(vals), _TYPE_FMT[typ]), *vals)
+    if typ in (_ASCII, _UNDEFINED):
+        return bytes(vals)
+    return struct.pack("<%d%s" % (len(vals), _TYPE_FMT[typ]), *vals)
+
+
+def _count(typ, vals):
+    """The TIFF count of `vals`: a RATIONAL is given as its numerator and denominator."""
+    return len(vals) // 2 if typ == _RATIONAL else len(vals)
 
 
 def _ifd_size(tags):
@@ -243,7 +256,7 @@ def _ifd(tags, at, next_ifd=0):
     blobs = b""
     for tag, typ, vals in tags:
         p = _payload(typ, vals)
-        count = len(vals)
+        count = _count(typ, vals)
         if len(p) <= 4:
             ifd += struct.pack("<HHI", tag, typ, count) + p.ljust(4, b"\0")
         else:
@@ -352,15 +365,42 @@ def cog_nodata(fmt, nodata):
         nodata, fmt, {"f32": "'nan'", "mask8": "0"}.get(fmt, "None")))
 
 
-def write_cog(path, data, tile_bytes, width, height, fmt, tile, geotransform, epsg=32632, nodata=None):
+_JPEG_SAMPLING = {"420": (2, 2), "444": (1, 1)}
+
+
+def write_cog(path, data, tile_bytes, width, height, fmt, tile, geotransform, epsg=32632, nodata=None,
+              compress="deflate", jpeg_tables=None, sampling="420", mask=None):
     """Writes Cloud-Optimized GeoTIFF tiles (GridMap.to_cog, cog_tiles; convention in include/aerial_mapper_b200.h,
     amb_cog_tiles_device) as a classic TIFF: the header, the IFD of level 0 at offset 8 and then those of the overviews
     in decreasing size, each followed by its out-of-line values, then the tile data in file order (the smallest level
     first, row-major within a level).  Every IFD has TileWidth = TileLength = tile, Compression 8 and the predictor of
     write_geotiff_strips; level 0 has NewSubfileType 0 and the georeferencing and GDAL_NODATA, each overview
     NewSubfileType 1.  nodata: see cog_nodata.  data: the tiles back to back; tile_bytes: each tile's length.  A file
-    over 4 GiB raises ValueError (no BigTIFF)."""
+    over 4 GiB raises ValueError (no BigTIFF).
+
+    compress="jpeg" (cog_jpeg_tiles; "gray8" and "bgr8" only, no nodata): Compression 7 with the JPEGTables stream
+    `jpeg_tables` on every image IFD, no Predictor; "bgr8" as Photometric 6 (YCbCr) with YCbCrSubSampling 2, 2 for
+    sampling "420" (1, 1 for "444") and ReferenceBlackWhite 0 255 128 255 128 255, "gray8" as Photometric 1.
+
+    mask=(data, tile_bytes) (cog_mask_tiles; "gray8" and "bgr8" only) adds GDAL's internal mask: after each level's IFD
+    the IFD of its mask, NewSubfileType 4 at level 0 and 5 on the overviews, Photometric 4, BitsPerSample 1, Compression
+    8 without a predictor, the same tiling; in the data each image tile is followed by its mask tile."""
+    if compress not in ("deflate", "jpeg"):
+        raise ValueError("write_cog: compress must be 'deflate' or 'jpeg', got %r" % (compress,))
+    jpeg = compress == "jpeg"
+    if jpeg or mask is not None:
+        if fmt not in ("gray8", "bgr8"):
+            raise ValueError("write_cog: %s is for 'gray8' and 'bgr8' only, got %r"
+                             % ("JPEG" if jpeg else "a mask", fmt))
     bands, bits, predictor = _DEFLATE_FORMATS[fmt]
+    if jpeg:
+        if nodata is not None:
+            raise ValueError("write_cog: a JPEG COG has no no-data value (JPEG is lossy): give a mask instead")
+        if sampling not in _JPEG_SAMPLING:
+            raise ValueError("write_cog: sampling must be '420' or '444', got %r" % (sampling,))
+        tables = bytes(jpeg_tables or b"")
+        if tables[:4] != b"\xff\xd8\xff\xdb" or tables[-2:] != b"\xff\xd9":
+            raise ValueError("write_cog: jpeg_tables must be a tables stream (SOI, DQT ..., DHT ..., EOI)")
     nd = cog_nodata(fmt, nodata)
     gt = _north_up(geotransform)
     data = memoryview(data).cast("B")
@@ -370,26 +410,61 @@ def write_cog(path, data, tile_bytes, width, height, fmt, tile, geotransform, ep
     if len(counts) != sum(n_tiles) or sum(counts) != len(data):
         raise ValueError("write_cog: %d tiles of %d bytes in all do not fit a %d x %d raster in tiles of %d (%d tiles)"
                          % (len(counts), sum(counts), width, height, tile, sum(n_tiles)))
+    if mask is not None:
+        mdata = memoryview(mask[0]).cast("B")
+        mcounts = [int(v) for v in mask[1]]
+        if len(mcounts) != len(counts) or sum(mcounts) != len(mdata):
+            raise ValueError("write_cog: %d mask tiles of %d bytes in all do not match the %d image tiles"
+                             % (len(mcounts), sum(mcounts), len(counts)))
     first = np.cumsum([0] + n_tiles[::-1])[::-1][1:]      # each level's first tile in file order (the smallest first)
-    tags = []
+    kw = {}
+    if jpeg:
+        extra = [(347, _UNDEFINED, list(tables))]
+        if bands == 3:
+            extra += [(530, _SHORT, list(_JPEG_SAMPLING[sampling])),
+                      (532, _RATIONAL, [0, 1, 255, 1, 128, 1, 255, 1, 128, 1, 255, 1])]
+        kw = {"compression": 7, "photometric": 6 if bands == 3 else 1, "extra": extra}
+    tags, kinds = [], []                                  # kinds: 0 image, 1 mask
     for k, (w, h) in enumerate(levels):
         c = counts[first[k]:first[k] + n_tiles[k]]
         layout = [(322, _LONG, [tile]), (323, _LONG, [tile]), (324, _LONG, [0] * len(c)), (325, _LONG, c)]
-        tags.append(_image_tags(w, h, bands, bits, predictor, layout, (gt, epsg, nd) if k == 0 else None,
-                                subfile=0 if k == 0 else 1))
+        tags.append(_image_tags(w, h, bands, bits, None if jpeg else predictor, layout,
+                                (gt, epsg, nd) if k == 0 else None, subfile=0 if k == 0 else 1, **kw))
+        kinds.append(0)
+        if mask is not None:
+            mc = mcounts[first[k]:first[k] + n_tiles[k]]
+            layout = [(322, _LONG, [tile]), (323, _LONG, [tile]), (324, _LONG, [0] * len(mc)), (325, _LONG, mc)]
+            tags.append(_image_tags(w, h, 1, 1, None, layout, subfile=4 if k == 0 else 5, compression=8,
+                                    photometric=4))
+            kinds.append(1)
     ifd_at = [8]
     for t in tags:
         ifd_at.append(ifd_at[-1] + _ifd_size(t))
     data_at = (ifd_at[-1] + 15) & ~15
-    _check_size(data_at + len(data))
-    starts = np.concatenate([[0], np.cumsum(np.asarray(counts, np.int64))[:-1]]) + data_at
+    total = len(data) + (len(mdata) if mask is not None else 0)
+    _check_size(data_at + total)
+    # file offsets of every tile (and mask tile), in file order: image tile i then its mask tile
+    step = np.asarray(counts, np.int64) + (np.asarray(mcounts, np.int64) if mask is not None else 0)
+    starts = np.concatenate([[0], np.cumsum(step)[:-1]]) + data_at
     head = b"II*\0" + struct.pack("<I", 8)
-    for k, t in enumerate(tags):
-        t = _set_tag(t, 324, _LONG, [int(v) for v in starts[first[k]:first[k] + n_tiles[k]]])
-        head += _ifd(t, ifd_at[k], ifd_at[k + 1] if k + 1 < len(tags) else 0)
+    for j, t in enumerate(tags):
+        k = j // 2 if mask is not None else j
+        s = starts[first[k]:first[k] + n_tiles[k]]
+        if kinds[j]:
+            s = s + np.asarray(counts[first[k]:first[k] + n_tiles[k]], np.int64)
+        t = _set_tag(t, 324, _LONG, [int(v) for v in s])
+        head += _ifd(t, ifd_at[j], ifd_at[j + 1] if j + 1 < len(tags) else 0)
     with open(path, "wb") as f:
         f.write(head + b"\0" * (data_at - len(head)))
-        f.write(data)
+        if mask is None:
+            f.write(data)
+        else:
+            at = mat = 0
+            for n, m in zip(counts, mcounts):
+                f.write(data[at:at + n])
+                f.write(mdata[mat:mat + m])
+                at += n
+                mat += m
 
 
 # ---- GeoTIFF reader: the subset GDAL writes for DEMs ----

@@ -644,6 +644,53 @@ int amb_cog_tiles_device(amb_ctx* ctx, const void* d_image, int32_t width, int32
 int amb_export_cog_tiles(amb_ctx* ctx, int layer, int format, int32_t tile, void* host_out, size_t capacity,
                          size_t* size, uint32_t* tile_bytes);
 
+/* ---- JPEG-compressed Cloud-Optimized GeoTIFF tiles, and 1-bit mask tiles ----
+ * Convention.  The image tiles of a tiled TIFF with Compression 7 (JPEG) and JPEGTables, the layout GDAL writes with
+ * COMPRESS=JPEG (PHOTOMETRIC=YCBCR for colour), for an AMB_RASTER_GRAY8 or AMB_RASTER_BGR8 raster.  Levels, reduction,
+ * T x T tiles with the part outside the level zero, and the order (the smallest level first) are those of
+ * amb_cog_tiles_device.
+ *   Image tile: an abbreviated JPEG stream SOI, SOF0 (T x T), SOS, entropy-coded data, EOI, with no APP0, DQT, DHT or
+ *     DRI.  Its entropy-coded data is exactly what cv2.imencode(".jpg", tile, [quality, sampling]) writes for the T x T
+ *     tile image (convention of amb_jpeg_encode_device: quality 1..100, sampling AMB_JPEG_420 or AMB_JPEG_444 for BGR8,
+ *     ignored for gray), so a tile is that file with its tables moved out.
+ *   Tables: one stream per file, SOI, the DQT segments, the DHT segments, EOI, with the bytes cv2.imencode writes: the
+ *     TIFF JPEGTables tag (347).  It depends on channels and quality only.
+ *   Mask tile (amb_cog_mask_tiles_device): GDAL's internal mask, for an AMB_RASTER_MASK8 raster (e.g. the export of
+ *     observation_index).  The pyramid is the MASK8 one (the maximum); every T x T tile is stored at 1 bit per pixel,
+ *     most significant bit first, 1 where the MASK8 byte is not 0 (valid), rows of T / 8 bytes, padding 0; each tile is
+ *     one zlib stream as in amb_cog_tiles_device but with no predictor (TIFF Predictor 1: libtiff has none for 1-bit
+ *     samples), so never longer than n + 5 ceil(n / 65535) + 6 bytes for n = T * T / 8.
+ * Inside, the stacked tiles are encoded as one JPEG image T wide and n_tiles * T high with a restart interval of
+ * (T / 8)^2 MCUs (gray, 4:4:4) or (T / 16)^2 (4:2:0): one interval per tile.  A restart resets the DC predictors and pads
+ * with 1 bits as the end of a separate stream does, so each interval's stuffed bytes are that tile's data.
+ * Errors: those of amb_cog_tiles_device; a format other than GRAY8 / BGR8 (JPEG) returns AMB_ERR_INVALID_ARGUMENT, a
+ * quality outside 1..100 or a bad sampling AMB_ERR_UNSUPPORTED.  Neither writes anything. */
+/* Host arithmetic, no GPU: a bound on the tiles' total size (headers, byte stuffing and EOI included); 0 if the
+ * arguments are invalid or unsupported. */
+size_t amb_cog_jpeg_max_size(int32_t width, int32_t height, int format, int32_t tile, int quality, int sampling);
+/* Host only, no GPU: the JPEGTables stream of channels 1 or 3 at `quality` into out (*size bytes, at most 600); a bad
+ * channels or quality returns AMB_ERR_UNSUPPORTED, capacity < *size AMB_ERR_SIZE_MISMATCH with the size in *size. */
+int amb_cog_jpeg_tables(int channels, int quality, void* out, size_t capacity, size_t* size);
+/* As amb_cog_tiles_device, JPEG tiles: on return the tiles are in host_out back to back in file order (*size bytes,
+ * pinned or pageable) and tile_bytes[] holds each tile's length.  If capacity < *size it returns AMB_ERR_SIZE_MISMATCH
+ * with the size needed in *size and writes nothing else.  Device scratch, kept by the context: the overview levels, the
+ * stacked tiles and the JPEG encoder's scratch for them (about 0.08 byte per stacked pixel at 4:2:0, 0.22 at 4:4:4,
+ * plus the compressed tiles twice). */
+int amb_cog_jpeg_tiles_device(amb_ctx* ctx, const void* d_image, int32_t width, int32_t height, size_t row_stride,
+                              int format, int32_t tile, int quality, int sampling, void* host_out, size_t capacity,
+                              size_t* size, uint32_t* tile_bytes);
+/* amb_export_raster_device of `layer` as GRAY8 or BGR8, then amb_cog_jpeg_tiles_device of the context's band. */
+int amb_export_cog_jpeg_tiles(amb_ctx* ctx, int layer, int format, int32_t tile, int quality, int sampling,
+                              void* host_out, size_t capacity, size_t* size, uint32_t* tile_bytes);
+/* Host arithmetic, no GPU: the sum of the mask tiles' bounds; 0 if the arguments are invalid or unsupported. */
+size_t amb_cog_mask_max_size(int32_t width, int32_t height, int32_t tile);
+/* The mask tiles of a MASK8 device raster (any byte alignment), with the contract of amb_cog_tiles_device. */
+int amb_cog_mask_tiles_device(amb_ctx* ctx, const void* d_mask, int32_t width, int32_t height, size_t row_stride,
+                              int32_t tile, void* host_out, size_t capacity, size_t* size, uint32_t* tile_bytes);
+/* amb_export_raster_device of `layer` as AMB_RASTER_MASK8, then amb_cog_mask_tiles_device of the context's band. */
+int amb_export_cog_mask_tiles(amb_ctx* ctx, int layer, int32_t tile, void* host_out, size_t capacity, size_t* size,
+                              uint32_t* tile_bytes);
+
 /* ---- measurement ---- */
 int amb_get_timings(amb_ctx* ctx, amb_timings* out);
 
