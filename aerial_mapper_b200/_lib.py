@@ -49,6 +49,17 @@ class Camera(C.Structure):
                 ("dist", C.c_double * 4), ("q_C_B", C.c_double * 4), ("t_C_B", C.c_double * 3)]
 
 
+# amb_sample_type of amb_tiff_layout, by numpy dtype name
+SAMPLE_TYPE = {"uint8": 0, "int16": 1, "uint16": 2, "int32": 3, "float32": 4, "float64": 5}
+
+
+class TiffLayout(C.Structure):
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("chunk_width", C.c_int32), ("chunk_height", C.c_int32),
+                ("tiled", C.c_int32), ("spp", C.c_int32), ("band", C.c_int32), ("sample", C.c_int32),
+                ("compression", C.c_int32), ("predictor", C.c_int32), ("n_chunks", C.c_uint32),
+                ("reserved_", C.c_uint32), ("offsets", C.c_void_p), ("byte_counts", C.c_void_p)]
+
+
 class Timings(C.Structure):
     _fields_ = [("dsm_h2d_ms", C.c_float), ("dsm_bin_ms", C.c_float), ("dsm_gather_ms", C.c_float),
                 ("dsm_fill_ms", C.c_float), ("dsm_total_ms", C.c_float), ("ortho_h2d_ms", C.c_float),
@@ -153,6 +164,12 @@ SYMBOLS = {
                                           C.c_int, C.c_float, C.c_int]),
     "amb_raster_import_tables": (C.c_int, [C.POINTER(Geometry), C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                            C.POINTER(C.c_double), C.c_int, _P, _P, _P, _P]),
+    "amb_tiff_decode_device": (C.c_int, [_P, _P, C.c_size_t, C.POINTER(TiffLayout), C.c_int32, C.c_int32, C.c_int32,
+                                         C.c_int32, _P, C.c_size_t]),
+    "amb_import_tiff": (C.c_int, [_P, C.c_int, _P, C.c_size_t, C.POINTER(TiffLayout), C.POINTER(C.c_double), C.c_int,
+                                  C.c_float, C.c_int]),
+    "amb_multi_import_tiff": (C.c_int, [_P, C.c_int, _P, C.c_size_t, C.POINTER(TiffLayout), C.POINTER(C.c_double),
+                                        C.c_int, C.c_float, C.c_int]),
     "amb_jpeg_max_size": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int, C.c_int, C.c_int, C.c_int32]),
     "amb_jpeg_encode_device": (C.c_int, [_P, _P, C.c_int32, C.c_int32, C.c_size_t, C.c_int, C.c_int, C.c_int,
                                          C.c_int32, _P, C.c_size_t, C.POINTER(C.c_size_t)]),

@@ -236,6 +236,28 @@ class GridMap(object):
                                       a.strides[0], gt, 0 if nodata is None else 1,
                                       0.0 if nodata is None else float(nodata), r), ctx)
 
+    def from_geotiff(self, name, path_or_bytes, band=0, overview=0, resample="bilinear", nodata="file"):
+        """from_raster of io.read_geotiff(path_or_bytes, band, overview) converted to float32, with its geotransform, bit
+        for bit, decoded on the device: only the strips or tiles the context's stripe reads are copied and inflated
+        (convention: include/aerial_mapper_b200.h, amb_import_tiff).  nodata: by default the file's GDAL_NODATA; None
+        for none.  A chunk of that window that does not inflate raises AmbError(AMB_ERR_CORRUPT_DATA) and the layer is
+        not written."""
+        if not self._resident:
+            raise AmbError(_lib.AMB_ERR_INVALID_ARGUMENT,
+                           "from_geotiff imports into device-resident layers: call to_device() first")
+        from . import io
+        r = _lib.RESAMPLE[resample] if isinstance(resample, str) else int(resample)
+        f = io._FileBytes(path_or_bytes)
+        t = io.tiff_layout(f.data, band, overview)
+        gt, _, file_nodata = t.georeferencing()
+        if isinstance(nodata, str) and nodata == "file":
+            nodata = file_nodata
+        L = t.c_layout()
+        ctx = self._ctx
+        check(lib().amb_import_tiff(ctx, LAYER_ID[name], C.c_void_p(f.file.ptr), f.file.size, C.byref(L),
+                                    (C.c_double * 6)(*gt), 0 if nodata is None else 1,
+                                    0.0 if nodata is None else float(nodata), r), ctx)
+
     def to_jpeg(self, name, quality=95, sampling="420", restart_interval=0, fmt=None):
         """The context's band of layer `name` as a baseline JPEG file (bytes), exported and encoded on the device
         (convention: include/aerial_mapper_b200.h, amb_jpeg_sampling), byte for byte cv2.imencode(".jpg", band, params)

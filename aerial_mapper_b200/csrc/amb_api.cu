@@ -385,7 +385,7 @@ void amb_destroy(amb_ctx* ctx) {
     if (ctx->layers[l]) cudaFree(ctx->layers[l]);
   DeviceBuffer* bufs[] = {&ctx->points,  &ctx->point_ids, &ctx->intensities, &ctx->records, &ctx->records_tmp, &ctx->tile_offsets, &ctx->point_order, &ctx->bucket_flags,
                             &ctx->bin_starts, &ctx->block_sums, &ctx->empty_cells,
-                          &ctx->counters, &ctx->dbg_count, &ctx->dbg_level,  &ctx->raster_band, &ctx->raster_taps, &ctx->jpeg_mcu, &ctx->jpeg_spine, &ctx->jpeg_words, &ctx->jpeg_out, &ctx->jdec_files, &ctx->jdec_stream, &ctx->jdec_meta, &ctx->jdec_subs, &ctx->jdec_coef, &ctx->deflate_scratch, &ctx->deflate_words, &ctx->cog_levels, &ctx->cog_tiles, &ctx->frames,     &ctx->frame_table,
+                          &ctx->counters, &ctx->dbg_count, &ctx->dbg_level,  &ctx->raster_band, &ctx->raster_taps, &ctx->jpeg_mcu, &ctx->jpeg_spine, &ctx->jpeg_words, &ctx->jpeg_out, &ctx->jdec_files, &ctx->jdec_stream, &ctx->jdec_meta, &ctx->jdec_subs, &ctx->jdec_coef, &ctx->deflate_scratch, &ctx->deflate_words, &ctx->cog_levels, &ctx->cog_tiles, &ctx->tiff_files, &ctx->tiff_inflated, &ctx->tiff_meta, &ctx->frames,     &ctx->frame_table,
                           &ctx->frame_cull, &ctx->frame_rects, &ctx->ortho_pix, &ctx->ortho_bbox};
   for (DeviceBuffer* b : bufs) b->release();
   for (int k = 0; k < EV_COUNT; ++k)

@@ -201,6 +201,9 @@ struct amb_ctx {
   amb::DeviceBuffer cog_levels;       // Cloud-Optimized GeoTIFF (raster_pyramid.cu): the overview levels 1.., rows padded
                                       // to 16 bytes, one after another
   amb::DeviceBuffer cog_tiles;        // ... every level's tiles stacked into one raster T wide, compressed as T-row strips
+  amb::DeviceBuffer tiff_files;       // TIFF chunk decoder (deflate_decode.cu): the file spans of a group's chunks
+  amb::DeviceBuffer tiff_inflated;    // ... their inflated bytes, then a 32 KB ring per stream
+  amb::DeviceBuffer tiff_meta;        // ... inflate and row jobs, per-stream status
   double dsm_density_hint = 0.0;  // points per cell of the whole cloud (0: derive from the points passed)
   bool dsm_debug = false;
   int dsm_stream_chunks = 4;  // (> 1, only with a host mirror of the output layer) gather + fill in column chunks, each chunk's
@@ -312,6 +315,11 @@ struct OrthoCall {
   const JpegFrame* headers = nullptr;      // JPEG: parsed by run_ortho
 };
 int ortho_run(amb_ctx* ctx, const OrthoCall& call);
+// deflate_decode.cu: the layout's argument checks (amb_tiff_decode_device), and image rows [r0, r1) x columns [c0, c1)
+// of a checked layout decoded into the device float32 band `out` (rows `stride` floats apart); synchronous
+int tiff_layout_check(const amb_tiff_layout* layout, size_t bytes);
+int tiff_decode_window(amb_ctx* ctx, const unsigned char* file, const amb_tiff_layout& layout, int32_t r0, int32_t r1,
+                       int32_t c0, int32_t c1, float* out, size_t stride);
 // amb_comm.cu: one step of a sharded cloud on a context of a communicator of several ranks (halo exchange, then
 // dsm_run over the rank's points and the neighbours' halos); records the DSM events and sets dsm_timed itself
 int sharded_step(amb_ctx* ctx, const double* d_xyz, const int* d_intensities, const uint64_t* d_ids, size_t n_local,

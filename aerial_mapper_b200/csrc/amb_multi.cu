@@ -155,6 +155,15 @@ int amb_multi_import_raster(amb_multi* m, int layer, const float* host_band, int
   });
 }
 
+int amb_multi_import_tiff(amb_multi* m, int layer, const void* file, size_t bytes, const amb_tiff_layout* layout,
+                          const double gt[6], int has_nodata, float nodata, int resample) {
+  if (!m) return AMB_ERR_INVALID_ARGUMENT;
+  // each stripe decodes the chunks of its own window; a corrupt one stops only that stripe's import
+  return for_each_stripe(m, [&](int, amb_ctx* c) {
+    return amb_import_tiff(c, layer, file, bytes, layout, gt, has_nodata, nodata, resample);
+  });
+}
+
 int amb_multi_set_host_mirror(amb_multi* m, int layer, float* host_full) {
   if (!m) return AMB_ERR_INVALID_ARGUMENT;
   for (size_t r = 0; r < m->ctx.size(); ++r) {

@@ -39,7 +39,6 @@ constexpr int kRecent = 8;                         // positions of a round searc
 constexpr int kChain = 4;                          // candidates tried per position
 constexpr int kNumLit = 286, kNumDist = 30, kNumSym = kNumLit + kNumDist;
 constexpr int kHeaderBytes = 576;                  // the largest dynamic header: 17 + 19 * 3 + 316 * 14 bits < 4608
-constexpr unsigned kAdlerMod = 65521u;
 // token words (uint16 per predicted byte): a token start holds 0x8000 | literal or 0x8100 + (length - 3), the byte
 // after a match start its distance - 1 (< 0x8000); every other byte kNone
 constexpr uint16_t kNone = 0xFFFFu, kLit = 0x8000u, kMatch = 0x8100u;
@@ -593,15 +592,11 @@ __global__ void __launch_bounds__(128)
     }
   }
   strip_bytes[strip] = 2 + (P + 7) / 8 + 4;
-  // Adler-32: a = 1 + sum b_i, b = n + sum (n - i) b_i (mod 65521); a segment at offset o adds (n - o) S - W
   const int ns = static_cast<int>((n + kSeg - 1) / kSeg);
   unsigned long long a = 1, bb = n % kAdlerMod;
   for (int q = 0; q < ns; ++q) {
     const int g = strip * s.segs + q;
-    const unsigned long long S = sums[2 * g] % kAdlerMod, W = sums[2 * g + 1] % kAdlerMod;
-    const unsigned long long rest = (n - static_cast<unsigned long long>(q) * kSeg) % kAdlerMod;
-    a = (a + S) % kAdlerMod;
-    bb = (bb + rest * S % kAdlerMod + kAdlerMod - W) % kAdlerMod;
+    adler_add_segment(n, static_cast<unsigned long long>(q) * kSeg, sums[2 * g], sums[2 * g + 1], &a, &bb);
   }
   adler[strip] = static_cast<uint32_t>((bb << 16) | a);
 }

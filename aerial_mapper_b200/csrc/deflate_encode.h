@@ -7,6 +7,21 @@
 
 namespace amb {
 
+constexpr unsigned kAdlerMod = 65521u;
+
+// Adler-32 of n bytes b_i from partial sums of segments: a = 1 + sum b_i, b = n + sum (n - i) b_i (mod 65521).  Start
+// with *a = 1, *b = n % 65521; a segment at offset o with S = sum b_i and W = sum (i - o) b_i over its bytes adds
+// (n - o) S - W to b.  The Adler-32 is (b << 16) | a.
+__host__ __device__ __forceinline__ void adler_add_segment(unsigned long long n, unsigned long long o,
+                                                           unsigned long long S, unsigned long long W,
+                                                           unsigned long long* a, unsigned long long* b) {
+  S %= kAdlerMod;
+  W %= kAdlerMod;
+  const unsigned long long rest = (n - o) % kAdlerMod;
+  *a = (*a + S) % kAdlerMod;
+  *b = (*b + rest * S % kAdlerMod + kAdlerMod - W) % kAdlerMod;
+}
+
 struct DeflateShape {
   const unsigned char* img;
   unsigned long long stride;     // bytes between raster rows

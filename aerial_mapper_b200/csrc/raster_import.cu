@@ -164,6 +164,19 @@ bool axis_window(const ImportTap* t, size_t n, int32_t* lo, int32_t* hi) {
   return *hi >= 0;
 }
 
+// The stripe's tables for a width x height raster and the window of raster columns [c_lo, c_hi] and rows [r_lo, r_hi]
+// they read, the tables rebased to the window's corner; false if the raster does not overlap the stripe
+bool import_window(const amb_ctx* ctx, int32_t width, int32_t height, const double* gt, int resample,
+                   std::vector<ImportTap>* taps, int32_t* c_lo, int32_t* c_hi, int32_t* r_lo, int32_t* r_hi) {
+  import_tables(ctx->geom, ctx->col_begin, ctx->col_end, width, height, gt, resample, taps);
+  const size_t rows = static_cast<size_t>(ctx->geom.rows);
+  if (!axis_window(taps->data(), rows, c_lo, c_hi) || !axis_window(taps->data() + rows, taps->size() - rows, r_lo, r_hi))
+    return false;
+  for (size_t k = 0; k < taps->size(); ++k)
+    if ((*taps)[k].k >= 0) (*taps)[k].k -= k < rows ? *c_lo : *r_lo;
+  return true;
+}
+
 // Enqueue the tables' upload and the kernel on the context's stream; band rows are `stride` floats apart.
 int import_enqueue(amb_ctx* ctx, int layer, const float* band, long long stride, const std::vector<ImportTap>& taps,
                    int has_nodata, float nodata, int resample) {
@@ -250,15 +263,10 @@ int amb_import_raster(amb_ctx* ctx, int layer, const float* host_band, int32_t w
     return AMB_ERR_INVALID_ARGUMENT;
   AMB_CUDA(ctx, cudaSetDevice(ctx->device));
   std::vector<ImportTap> taps;
-  import_tables(ctx->geom, ctx->col_begin, ctx->col_end, width, height, gt, resample, &taps);
   int32_t c_lo, c_hi, r_lo, r_hi;
-  const size_t rows = static_cast<size_t>(ctx->geom.rows);
-  if (!axis_window(taps.data(), rows, &c_lo, &c_hi) ||
-      !axis_window(taps.data() + rows, taps.size() - rows, &r_lo, &r_hi))
+  if (!import_window(ctx, width, height, gt, resample, &taps, &c_lo, &c_hi, &r_lo, &r_hi))
     return AMB_OK;  // no overlap with the stripe
   // only the window crosses PCIe, packed: the tables index it from its corner
-  for (size_t k = 0; k < taps.size(); ++k)
-    if (taps[k].k >= 0) taps[k].k -= k < rows ? c_lo : r_lo;
   const size_t win_w = static_cast<size_t>(c_hi - c_lo + 1), win_h = static_cast<size_t>(r_hi - r_lo + 1);
   AMB_CUDA(ctx, ctx->raster_band.reserve(win_w * win_h * sizeof(float)));
   const StagedRect rect{ctx->raster_band.as<unsigned char>(), win_w * sizeof(float),
@@ -271,6 +279,29 @@ int amb_import_raster(amb_ctx* ctx, int layer, const float* host_band, int32_t w
                       resample);
   if (st != AMB_OK) return st;
   AMB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // the caller's band (pinned: read by the DMA) may be reused
+  return AMB_OK;
+}
+
+int amb_import_tiff(amb_ctx* ctx, int layer, const void* file, size_t bytes, const amb_tiff_layout* layout,
+                    const double gt[6], int has_nodata, float nodata, int resample) {
+  if (!ctx || !file || tiff_layout_check(layout, bytes) != AMB_OK ||
+      !import_args_ok(layer, layout->width, layout->height, 4 * static_cast<size_t>(layout->width), gt, resample))
+    return AMB_ERR_INVALID_ARGUMENT;
+  AMB_CUDA(ctx, cudaSetDevice(ctx->device));
+  std::vector<ImportTap> taps;
+  int32_t c_lo, c_hi, r_lo, r_hi;
+  if (!import_window(ctx, layout->width, layout->height, gt, resample, &taps, &c_lo, &c_hi, &r_lo, &r_hi))
+    return AMB_OK;  // no overlap with the stripe
+  // only the window's chunks are copied and decoded, into the window band the tables index from its corner
+  const size_t win_w = static_cast<size_t>(c_hi - c_lo + 1), win_h = static_cast<size_t>(r_hi - r_lo + 1);
+  AMB_CUDA(ctx, ctx->raster_band.reserve(win_w * win_h * sizeof(float)));
+  int st = tiff_decode_window(ctx, static_cast<const unsigned char*>(file), *layout, r_lo, r_hi + 1, c_lo, c_hi + 1,
+                              ctx->raster_band.as<float>(), win_w);
+  if (st != AMB_OK) return st;
+  st = import_enqueue(ctx, layer, ctx->raster_band.as<float>(), static_cast<long long>(win_w), taps, has_nodata, nodata,
+                      resample);
+  if (st != AMB_OK) return st;
+  AMB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return AMB_OK;
 }
 

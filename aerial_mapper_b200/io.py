@@ -12,7 +12,8 @@ and the output side ("next" row N4):
     write_geotiff                   :349-509   toGeoTiff / writeDataToDEMGeoTiffColor, with the map's geotransform
     write_geotiff_strips                        the same tags around Deflate strips compressed on the device
 
-and back in: read_geotiff, the DEM GeoTIFFs GDAL writes (GridMap.from_raster resamples them into a layer).
+and back in: read_geotiff, the DEM GeoTIFFs GDAL writes (GridMap.from_raster resamples them into a layer), and
+read_geotiff_device, the same files decoded on a GPU (GridMap.from_geotiff imports them straight from the file).
 """
 import ctypes as C
 import math
@@ -619,9 +620,63 @@ def read_geotiff(path, band=0, overview=0):
     are the first IFD's.  An overview the file does not have raises ValueError.
 
     For GridMap.from_raster a DEM is converted with a.astype(np.float32), its no-data value passed along: that value must
-    be exact in float32 (true of every int16 and uint16 value) or pixels holding it will not compare equal."""
+    be exact in float32 (true of every int16 and uint16 value) or pixels holding it will not compare equal.
+
+    read_geotiff_device reads the same files on a GPU."""
     with open(path, "rb") as f:
         data = f.read()
+    t = tiff_layout(data, band, overview)
+    out = np.empty((t.height, t.width), t.dtype)
+    for (r0, c0, rows, cols), at, n in zip(t.grid, t.offsets, t.counts):
+        if r0 >= t.height or c0 >= t.width:
+            continue
+        chunk = data[at:at + n]
+        if t.compression != 1:
+            chunk = zlib.decompress(chunk)
+        a = _undo_predictor(chunk, t.predictor, t.dtype, rows, cols, t.spp)
+        out[r0:r0 + rows, c0:c0 + cols] = a[:t.height - r0, :t.width - c0, band]
+    return (out,) + t.georeferencing()
+
+
+class TiffLayout(object):
+    """One image of a TIFF as read_geotiff reads it (tiff_layout): its size, samples, compression and predictor, and its
+    chunks: grid [(row, column, rows, columns)] of every strip or tile (full tiles at the edges, the last strip short),
+    offsets and counts into the file.  base: the first IFD's tags, tags: the image's own."""
+
+    def __init__(self, **kw):
+        self.__dict__.update(kw)
+
+    def georeferencing(self):
+        """(GDAL geotransform, EPSG code or None, no-data value or None) of the image, as read_geotiff returns them: an
+        overview's pixel sizes are the first IFD's scaled by W / w_k and H / h_k."""
+        base = self.base
+        keys = _geokeys(base)
+        epsg = keys.get(3072, keys.get(2048))
+        nodata = base.get(42113)
+        gt = _geotransform(base)
+        if self.overview:
+            sx, sy = base[256][0] / self.width, base[257][0] / self.height
+            gt = (gt[0], gt[1] * sx, gt[2], gt[3], gt[4], gt[5] * sy)
+        return gt, (None if epsg in (None, 0, 32767) else int(epsg)), (None if nodata is None else float(nodata.strip()))
+
+    def c_layout(self):
+        """The amb_tiff_layout of the image's grid of chunks (the arrays it points to live as long as the result)."""
+        n = len(self.grid)
+        if min(len(self.offsets), len(self.counts)) < n:
+            raise ValueError("read_geotiff_device: %d chunk offsets and %d byte counts for a grid of %d chunks"
+                             % (len(self.offsets), len(self.counts), n))
+        offsets = np.asarray(self.offsets[:n], np.uint64)
+        counts = np.asarray(self.counts[:n], np.uint64)
+        L = _lib.TiffLayout(self.width, self.height, self.chunk_width, self.chunk_height, int(self.tiled), self.spp,
+                            self.band, _lib.SAMPLE_TYPE[np.dtype(self.dtype).name], self.compression, self.predictor, n,
+                            0, offsets.ctypes.data, counts.ctypes.data)
+        L._keep = (offsets, counts)
+        return L
+
+
+def tiff_layout(data, band=0, overview=0):
+    """The TiffLayout of band `band` of image `overview` of the TIFF file `data` (bytes), with read_geotiff's checks:
+    anything it does not read raises ValueError naming the tag and value."""
     if isinstance(overview, bool) or not isinstance(overview, (int, np.integer)) or overview < 0:
         raise ValueError("read_geotiff: overview must be a non-negative integer, got %r" % (overview,))
     base = tags = _read_ifd(data)
@@ -652,27 +707,56 @@ def read_geotiff(path, band=0, overview=0):
         offsets, counts = tags[324], tags[325]
         across = (width + tw - 1) // tw
         grid = [((k // across) * th, (k % across) * tw, th, tw) for k in range(len(offsets))]
+        tiled, cw, ch = True, tw, th
     elif 273 in tags:                                   # strips
         rps = min(tags.get(278, (height,))[0], height)
         offsets, counts = tags[273], tags[279]
         grid = [(k * rps, 0, min(rps, height - k * rps), width) for k in range(len(offsets))]
+        tiled, cw, ch = False, width, rps
     else:
         raise ValueError("read_geotiff: neither strips nor tiles")
-    out = np.empty((height, width), dtype)
-    for (r0, c0, rows, cols), at, n in zip(grid, offsets, counts):
-        if r0 >= height or c0 >= width:
-            continue
-        chunk = data[at:at + n]
-        if comp != 1:
-            chunk = zlib.decompress(chunk)
-        a = _undo_predictor(chunk, predictor, dtype, rows, cols, spp)
-        out[r0:r0 + rows, c0:c0 + cols] = a[:height - r0, :width - c0, band]
-    keys = _geokeys(base)
-    epsg = keys.get(3072, keys.get(2048))
-    nodata = base.get(42113)
-    gt = _geotransform(base)
-    if overview:
-        sx, sy = base[256][0] / width, base[257][0] / height
-        gt = (gt[0], gt[1] * sx, gt[2], gt[3], gt[4], gt[5] * sy)
-    return out, gt, (None if epsg in (None, 0, 32767) else int(epsg)), \
-        (None if nodata is None else float(nodata.strip()))
+    n_grid = -(-height // ch) * (-(-width // cw) if tiled else 1)
+    return TiffLayout(base=base, tags=tags, overview=int(overview), width=width, height=height, spp=spp, band=band,
+                      dtype=dtype, compression=comp, predictor=predictor, tiled=tiled, chunk_width=cw, chunk_height=ch,
+                      offsets=offsets, counts=counts, grid=grid[:n_grid] if len(grid) >= n_grid else grid)
+
+
+class _FileBytes(object):
+    """A TIFF file handed to the library without copying it: a path is read once, bytes and bytearray are used in
+    place, any other bytes-like object is copied once."""
+
+    def __init__(self, path_or_bytes):
+        from .api import _JpegFile
+        if isinstance(path_or_bytes, (str, os.PathLike)):
+            with open(path_or_bytes, "rb") as f:
+                path_or_bytes = f.read()
+        elif not isinstance(path_or_bytes, (bytes, bytearray)):
+            path_or_bytes = bytes(memoryview(path_or_bytes).cast("B"))
+        self.data = path_or_bytes
+        self.file = _JpegFile(path_or_bytes)
+
+
+def _decode_device(f, t, device):
+    """Image `t` (a TiffLayout of the file f, a _FileBytes) decoded on a GPU: torch CUDA float32 [H, W]."""
+    import torch
+    from .api import _jpeg_context
+    dev = torch.device("cuda", int(device))
+    out = torch.empty((t.height, t.width), dtype=torch.float32, device=dev)
+    L = t.c_layout()
+    ctx = _jpeg_context(int(device))
+    torch.cuda.synchronize(dev)   # the output's allocation is ordered before the decode on the context's stream
+    _lib.check(_lib.lib().amb_tiff_decode_device(ctx, C.c_void_p(f.file.ptr), f.file.size, C.byref(L), 0, t.height, 0,
+                                                 t.width, C.c_void_p(out.data_ptr()), 4 * t.width), ctx)
+    return out
+
+
+def read_geotiff_device(path_or_bytes, band=0, overview=0, device=0):
+    """read_geotiff on a GPU: (torch CUDA float32 [H, W], geotransform, EPSG code or None, no-data value or None), the
+    array bit for bit read_geotiff(...)[0].astype(np.float32) (a NaN of a float64 file stays a NaN, its payload is not
+    promised).  The file's chunks are inflated, unpredicted and converted on the device (convention in
+    include/aerial_mapper_b200.h, amb_tiff_decode_device); the IFD is parsed here, with read_geotiff's ValueErrors.  A
+    chunk that does not inflate raises AmbError(AMB_ERR_CORRUPT_DATA)."""
+    f = _FileBytes(path_or_bytes)
+    t = tiff_layout(f.data, band, overview)
+    geo = t.georeferencing()
+    return (_decode_device(f, t, device),) + geo

@@ -44,7 +44,8 @@ typedef enum amb_status {
   AMB_ERR_CHECK_FAILED = -6,     /* reference CHECK(alpha > 0.0), ortho-backward-grid.cc:178 */
   AMB_ERR_NO_DEVICE = -7,
   AMB_ERR_UNSUPPORTED = -8,
-  AMB_ERR_CORRUPT_DATA = -9      /* a JPEG scan that is not valid for its header (amb_jpeg_decode_device) */
+  AMB_ERR_CORRUPT_DATA = -9      /* a JPEG scan that is not valid for its header (amb_jpeg_decode_device), or a TIFF
+                                    chunk that does not inflate to its data (amb_tiff_decode_device) */
 } amb_status;
 
 /* Geometry of the grid_map (grid_map::GridMap::setGeometry as called at aerial-mapper-grid-map.cc:30-33). */
@@ -495,6 +496,68 @@ int amb_multi_import_raster(amb_multi* m, int layer, const float* host_band, int
 int amb_raster_import_tables(const amb_geometry* geom, int32_t col_begin, int32_t col_end, int32_t width, int32_t height,
                              const double gt[6], int resample, int32_t* src_col, double* fx, int32_t* src_row,
                              double* fy);
+
+/* ---- import of a Deflate-compressed (or uncompressed) TIFF band, inflated on the device ----
+ * Convention.  One image (IFD) of a classic little-endian TIFF, described by amb_tiff_layout (the caller parses the
+ * TIFF; the library never does): strips or tiles, PlanarConfiguration 1, Compression 1, 8 or 32946, Predictor 1, 2
+ * (integer samples) or 3 (floating point), uint8, int16, uint16, int32, float32 or float64 samples, `spp` samples per
+ * pixel of which band `band` is read.  The result is, bit for bit, the band as float32 the way numpy converts it
+ * (a.astype(np.float32)): float32 samples are moved as bits (NaN payloads and -0 survive), int32 and float64 round to
+ * nearest even, a float64 NaN stays a NaN (its payload is not promised).
+ *   Chunks: chunk k of a tiled image is the tile at rows (k / across) * chunk_height, columns (k % across) *
+ *     chunk_width (across = ceil(width / chunk_width)), every tile chunk_width x chunk_height pixels, the parts outside
+ *     the image ignored; chunk k of a striped image (chunk_width == width) holds rows [k * chunk_height, + chunk_height)
+ *     cut at the image's height.  A chunk's expected bytes are its rows x chunk_width x spp x the sample's bytes.
+ *   Compressed chunk: one zlib stream (RFC 1950: CM 8, CINFO <= 7, a valid FCHECK, no preset dictionary) of RFC 1951
+ *     stored, fixed and dynamic blocks, accepted as zlib.decompress accepts it: the stream must reach its final block
+ *     and a correct Adler-32; bytes after the stream are ignored; it must inflate to at least the expected bytes, and
+ *     bytes past them are ignored.  An uncompressed chunk must hold at least the expected bytes.
+ *   Predictor, per predictor row (a tile row for tiles, an image row for strips): 2 adds each sample to the one spp
+ *     samples before it, modulo the sample type; 3 (libtiff's floating-point predictor, the inverse of
+ *     amb_deflate_strips_device's) adds each byte to the byte spp before it mod 256, over the row's big-endian byte
+ *     planes, most significant plane first, then reassembles the samples.
+ *   Corruption: a chunk that zlib.decompress would reject (a bad header, block type 3, an over-subscribed or incomplete
+ *     code, a distance before the start of the output, a truncated stream, a wrong Adler-32, too few bytes) returns
+ *     AMB_ERR_CORRUPT_DATA and nothing is written.  Only the chunks that intersect the rows and columns asked for are
+ *     copied to the device and inflated: the others are never read, so their corruption is never seen.
+ * Argument errors (AMB_ERR_INVALID_ARGUMENT, before anything is copied): a NULL pointer; width, height, chunk sides or
+ * spp < 1; a band outside [0, spp); an unknown sample type, compression or predictor, or predictor 2 with float or 3
+ * with integer samples; strips with chunk_width != width; n_chunks other than the chunk grid's count; a chunk whose
+ * offset + byte count passes `bytes`; a chunk of more than 2^32 expected bytes.
+ * Scratch, kept by the context: the window's float32 band, and chunks in groups whose compressed, inflated and 32 KB
+ * window bytes stay under 1 GiB (a chunk that alone needs more forms a group of its own).
+ * One warp inflates one zlib stream: an image stored as one strip inflates on one warp, slower than a host thread. */
+typedef enum amb_sample_type {
+  AMB_SAMPLE_U8 = 0, AMB_SAMPLE_I16 = 1, AMB_SAMPLE_U16 = 2, AMB_SAMPLE_I32 = 3, AMB_SAMPLE_F32 = 4, AMB_SAMPLE_F64 = 5
+} amb_sample_type;
+typedef struct amb_tiff_layout {
+  int32_t width, height;             /* pixels */
+  int32_t chunk_width, chunk_height; /* TileWidth x TileLength, or width x RowsPerStrip */
+  int32_t tiled;                     /* 1: tiles, 0: strips */
+  int32_t spp, band;                 /* samples per pixel, the one read */
+  int32_t sample;                    /* amb_sample_type */
+  int32_t compression;               /* 1, 8 or 32946 */
+  int32_t predictor;                 /* 1, 2 or 3 */
+  uint32_t n_chunks;
+  uint32_t reserved_;
+  const uint64_t* offsets;           /* [n_chunks]: StripOffsets / TileOffsets, into the file */
+  const uint64_t* byte_counts;       /* [n_chunks]: StripByteCounts / TileByteCounts */
+} amb_tiff_layout;
+/* Decodes image rows [r0, r1) and columns [c0, c1) (0 <= r0 < r1 <= height, 0 <= c0 < c1 <= width) of the band into the
+ * device float32 band d_band valid on the context's device (row r - r0 at d_band + (r - r0) * row_stride bytes, a
+ * multiple of 4 of at least 4 (c1 - c0)), ordered after earlier work on the context's stream.  file: the whole file,
+ * `bytes` long, in host memory (pinned or pageable).  Synchronous: corruption is found on the device. */
+int amb_tiff_decode_device(amb_ctx* ctx, const void* file, size_t bytes, const amb_tiff_layout* layout, int32_t r0,
+                           int32_t r1, int32_t c0, int32_t c1, float* d_band, size_t row_stride);
+/* amb_import_raster of the decoded band (width x height, geotransform gt) with the same arguments and the same result:
+ * only the window of rows and columns the stripe's import tables reference is decoded, so only the chunks it meets are
+ * copied and inflated.  No overlap with the stripe: AMB_OK, nothing copied.  Returns when `file` may be reused. */
+int amb_import_tiff(amb_ctx* ctx, int layer, const void* file, size_t bytes, const amb_tiff_layout* layout,
+                    const double gt[6], int has_nodata, float nodata, int resample);
+/* Every stripe of amb_multi decodes and imports its own window, all devices at once; a stripe whose window holds a
+ * corrupt chunk leaves its layer untouched.  Returns the first stripe's non-OK status. */
+int amb_multi_import_tiff(amb_multi* m, int layer, const void* file, size_t bytes, const amb_tiff_layout* layout,
+                          const double gt[6], int has_nodata, float nodata, int resample);
 
 /* ---- baseline JPEG of an 8-bit raster ----
  * Convention.  The file is byte for byte what libjpeg(-turbo) writes (OpenCV cv2.imencode(".jpg", img, params)) for the
