@@ -170,6 +170,19 @@ SYMBOLS = {
                                   C.c_float, C.c_int]),
     "amb_multi_import_tiff": (C.c_int, [_P, C.c_int, _P, C.c_size_t, C.POINTER(TiffLayout), C.POINTER(C.c_double),
                                         C.c_int, C.c_float, C.c_int]),
+    "amb_import_raster_lonlat": (C.c_int, [_P, C.c_int, _P, C.c_int32, C.c_int32, C.c_size_t, C.POINTER(C.c_double),
+                                           C.c_int, C.c_float, C.c_int, C.c_int32]),
+    "amb_import_raster_lonlat_device": (C.c_int, [_P, C.c_int, _P, C.c_int32, C.c_int32, C.c_size_t,
+                                                  C.POINTER(C.c_double), C.c_int, C.c_float, C.c_int, C.c_int32]),
+    "amb_multi_import_raster_lonlat": (C.c_int, [_P, C.c_int, _P, C.c_int32, C.c_int32, C.c_size_t,
+                                                 C.POINTER(C.c_double), C.c_int, C.c_float, C.c_int, C.c_int32]),
+    "amb_import_tiff_lonlat": (C.c_int, [_P, C.c_int, _P, C.c_size_t, C.POINTER(TiffLayout), C.POINTER(C.c_double),
+                                         C.c_int, C.c_float, C.c_int, C.c_int32]),
+    "amb_multi_import_tiff_lonlat": (C.c_int, [_P, C.c_int, _P, C.c_size_t, C.POINTER(TiffLayout),
+                                               C.POINTER(C.c_double), C.c_int, C.c_float, C.c_int, C.c_int32]),
+    "amb_lonlat_import_window": (C.c_int, [C.POINTER(Geometry), C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                           C.POINTER(C.c_double), _P]),
+    "amb_lonlat_positions_device": (C.c_int, [_P, C.c_int32, _P]),
     "amb_jpeg_max_size": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int, C.c_int, C.c_int, C.c_int32]),
     "amb_jpeg_encode_device": (C.c_int, [_P, _P, C.c_int32, C.c_int32, C.c_size_t, C.c_int, C.c_int, C.c_int,
                                          C.c_int32, _P, C.c_size_t, C.POINTER(C.c_size_t)]),

@@ -236,12 +236,35 @@ class GridMap(object):
                                       a.strides[0], gt, 0 if nodata is None else 1,
                                       0.0 if nodata is None else float(nodata), r), ctx)
 
-    def from_geotiff(self, name, path_or_bytes, band=0, overview=0, resample="bilinear", nodata="file"):
+    def from_lonlat_raster(self, name, band, geotransform, map_epsg, nodata=None, resample="bilinear"):
+        """from_raster of a longitude/latitude raster (WGS84, EPSG:4326; geotransform (lon0, dlon, 0, lat0, 0, -dlat) in
+        degrees) into a map in the WGS84 UTM zone `map_epsg` (32601-32660 or 32701-32760): every cell is
+        inverse-projected on the device, then resampled by from_raster's rule (convention: include/aerial_mapper_b200.h,
+        amb_import_raster_lonlat).  Heights are imported as stored: no datum shift, no geoid correction."""
+        if not self._resident:
+            raise AmbError(_lib.AMB_ERR_INVALID_ARGUMENT,
+                           "from_lonlat_raster imports into device-resident layers: call to_device() first")
+        r = _lib.RESAMPLE[resample] if isinstance(resample, str) else int(resample)
+        a = np.asarray(band)
+        if a.ndim != 2 or a.dtype != np.float32 or a.strides[1] != 4 or a.strides[0] < 4 * a.shape[1]:
+            raise AmbError(_lib.AMB_ERR_INVALID_ARGUMENT,
+                           "band must be float32 [H, W] with unit element stride and increasing rows; got %s %r strides %r"
+                           % (a.dtype, a.shape, a.strides))
+        gt = (C.c_double * 6)(*[float(v) for v in geotransform])
+        ctx = self._ctx
+        check(lib().amb_import_raster_lonlat(ctx, LAYER_ID[name], a.ctypes.data_as(C.c_void_p), a.shape[1], a.shape[0],
+                                             a.strides[0], gt, 0 if nodata is None else 1,
+                                             0.0 if nodata is None else float(nodata), r, int(map_epsg)), ctx)
+
+    def from_geotiff(self, name, path_or_bytes, band=0, overview=0, resample="bilinear", nodata="file", map_epsg=None):
         """from_raster of io.read_geotiff(path_or_bytes, band, overview) converted to float32, with its geotransform, bit
         for bit, decoded on the device: only the strips or tiles the context's stripe reads are copied and inflated
         (convention: include/aerial_mapper_b200.h, amb_import_tiff).  nodata: by default the file's GDAL_NODATA; None
         for none.  A chunk of that window that does not inflate raises AmbError(AMB_ERR_CORRUPT_DATA) and the layer is
-        not written."""
+        not written.
+        map_epsg: None reads the file as in the map's frame, whatever its EPSG code.  Given (the map's UTM zone, e.g.
+        32632), a file in EPSG:4326 is imported as from_lonlat_raster of its array, one in map_epsg as above, and any
+        other file (another code, or none) raises ValueError."""
         if not self._resident:
             raise AmbError(_lib.AMB_ERR_INVALID_ARGUMENT,
                            "from_geotiff imports into device-resident layers: call to_device() first")
@@ -249,14 +272,18 @@ class GridMap(object):
         r = _lib.RESAMPLE[resample] if isinstance(resample, str) else int(resample)
         f = io._FileBytes(path_or_bytes)
         t = io.tiff_layout(f.data, band, overview)
-        gt, _, file_nodata = t.georeferencing()
+        gt, file_epsg, file_nodata = t.georeferencing()
+        lonlat = _lonlat_source(file_epsg, map_epsg)
         if isinstance(nodata, str) and nodata == "file":
             nodata = file_nodata
         L = t.c_layout()
         ctx = self._ctx
-        check(lib().amb_import_tiff(ctx, LAYER_ID[name], C.c_void_p(f.file.ptr), f.file.size, C.byref(L),
-                                    (C.c_double * 6)(*gt), 0 if nodata is None else 1,
-                                    0.0 if nodata is None else float(nodata), r), ctx)
+        args = (ctx, LAYER_ID[name], C.c_void_p(f.file.ptr), f.file.size, C.byref(L), (C.c_double * 6)(*gt),
+                0 if nodata is None else 1, 0.0 if nodata is None else float(nodata), r)
+        if lonlat:
+            check(lib().amb_import_tiff_lonlat(*(args + (int(map_epsg),))), ctx)
+        else:
+            check(lib().amb_import_tiff(*args), ctx)
 
     def to_jpeg(self, name, quality=95, sampling="420", restart_interval=0, fmt=None):
         """The context's band of layer `name` as a baseline JPEG file (bytes), exported and encoded on the device
@@ -384,6 +411,21 @@ class GridMap(object):
             self._free_pinned()
         except Exception:
             pass
+
+
+def _lonlat_source(file_epsg, map_epsg):
+    """Whether from_geotiff(map_epsg=...) reads a file of EPSG code file_epsg as a longitude/latitude raster."""
+    if map_epsg is None:
+        return False
+    map_epsg = int(map_epsg)
+    if not (32601 <= map_epsg <= 32660 or 32701 <= map_epsg <= 32760):
+        raise ValueError("from_geotiff: map_epsg %d is not a WGS84 UTM zone (32601-32660, 32701-32760)" % map_epsg)
+    if file_epsg == 4326:
+        return True
+    if file_epsg == map_epsg:
+        return False
+    raise ValueError("from_geotiff: the file is in EPSG:%s, the map in EPSG:%d; only EPSG:4326 files or files in the "
+                     "map's own zone are imported" % ("none" if file_epsg is None else file_epsg, map_epsg))
 
 
 class AerialGridMap(object):

@@ -100,6 +100,7 @@ enum CounterSlot {
   CTR_ORTHO_CHECK = 8,     // sticky: CHECK(alpha > 0.0), ortho-backward-grid.cc:178
   CTR_PCL_CELLS = 10,      // adaptive OrthoFromPcl: cells listed for the 10^k radius growth
   CTR_PCL_UNRESOLVED = 11, // adaptive OrthoFromPcl: cells no level could fill
+  CTR_LONLAT_OUTSIDE = 12, // longitude/latitude import: a tap fell outside the copied raster window (reset per call)
   CTR_COUNT = 16
 };
 
@@ -185,7 +186,7 @@ struct amb_ctx {
   amb::DeviceBuffer dbg_level;    // int8 per slab cell
   amb::DeviceBuffer raster_band;  // amb_export_raster: the converted band before its copy to the host;
                                   // amb_import_raster: the raster window after its copy to the device
-  amb::DeviceBuffer raster_taps;  // amb_import_raster*: the per-axis tables of the last import
+  amb::DeviceBuffer raster_taps;  // amb_import_raster* / amb_import_*_lonlat: the per-axis tables of the last import
   amb::DeviceBuffer jpeg_mcu;     // JPEG encoder (jpeg_encode.cu): DC per block, bit offset per MCU, byte offset per interval
   amb::DeviceBuffer jpeg_spine;   // ... tile sums of its scans
   amb::DeviceBuffer jpeg_words;   // ... the entropy-coded stream before byte stuffing, and 0xFF counts per chunk

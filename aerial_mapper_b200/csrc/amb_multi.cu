@@ -164,6 +164,24 @@ int amb_multi_import_tiff(amb_multi* m, int layer, const void* file, size_t byte
   });
 }
 
+int amb_multi_import_raster_lonlat(amb_multi* m, int layer, const float* host_band, int32_t width, int32_t height,
+                                   size_t row_stride, const double gt[6], int has_nodata, float nodata, int resample,
+                                   int32_t map_epsg) {
+  if (!m) return AMB_ERR_INVALID_ARGUMENT;
+  return for_each_stripe(m, [&](int, amb_ctx* c) {
+    return amb_import_raster_lonlat(c, layer, host_band, width, height, row_stride, gt, has_nodata, nodata, resample,
+                                    map_epsg);
+  });
+}
+
+int amb_multi_import_tiff_lonlat(amb_multi* m, int layer, const void* file, size_t bytes, const amb_tiff_layout* layout,
+                                 const double gt[6], int has_nodata, float nodata, int resample, int32_t map_epsg) {
+  if (!m) return AMB_ERR_INVALID_ARGUMENT;
+  return for_each_stripe(m, [&](int, amb_ctx* c) {
+    return amb_import_tiff_lonlat(c, layer, file, bytes, layout, gt, has_nodata, nodata, resample, map_epsg);
+  });
+}
+
 int amb_multi_set_host_mirror(amb_multi* m, int layer, float* host_full) {
   if (!m) return AMB_ERR_INVALID_ARGUMENT;
   for (size_t r = 0; r < m->ctx.size(); ++r) {

@@ -559,6 +559,54 @@ int amb_import_tiff(amb_ctx* ctx, int layer, const void* file, size_t bytes, con
 int amb_multi_import_tiff(amb_multi* m, int layer, const void* file, size_t bytes, const amb_tiff_layout* layout,
                           const double gt[6], int has_nodata, float nodata, int resample);
 
+/* ---- import of a longitude/latitude raster into a UTM map, every cell inverse-projected on the device ----
+ * Frames.  The map's frame is a WGS84 UTM zone named by its EPSG code map_epsg: 32601-32660 (north, false northing 0)
+ * or 32701-32760 (south, false northing 10^7).  A cell's position is amb_geometry_position's (easting, northing in that
+ * zone, false easting and false northing included), exactly as amb_raster_geotransform states it.  The raster's frame is
+ * geographic WGS84 (EPSG:4326): x = longitude, y = latitude, in degrees, with a north-up geotransform
+ * (lon0, dlon, 0, lat0, 0, -dlat) and PixelIsArea pixels (read_geotiff already shifts a PixelIsPoint file's).  Any other
+ * map_epsg, ETRS89, NAD83 and national grids included, returns AMB_ERR_INVALID_ARGUMENT.
+ * Projection.  The inverse transverse Mercator as Krüger's series of order 6 in n (Karney 2011, "Transverse Mercator
+ * with an accuracy of a few nanometers"; what PROJ and GeographicLib use) with a = 6378137, f = 1/298.257223563,
+ * k0 = 0.9996, FE = 500000, lambda0 = 6 zone - 183 degrees; the conformal latitude goes to the geodetic one by two Newton
+ * steps on tan(phi).  Every cell's (lon, lat) is within 1e-11 degrees (about 1 um) of a high-precision evaluation of the
+ * same series, which is itself within a few nm of the exact projection within 3900 km of the central meridian.
+ * Resampling.  Per cell, u = (lon - gt0) / gt1 and v = (lat - gt3) / gt5, each one IEEE double subtraction and one
+ * division, no contraction; from (u, v) on, amb_resample's rule with u_i, v_j replaced by the cell's u, v: the same
+ * coverage, taps, 2^-20 snap, rounded double blend, no-data and untouched cells.
+ * Window.  For a host band or a TIFF, the host computes the raster window the stripe reads from the boundary cells of its
+ * rectangle (longitude and isometric latitude are harmonic in easting and northing, so their extremes lie on the
+ * boundary), one pixel wider on each side, clamped to the raster; only that window is copied (host band) or decoded
+ * (TIFF).  A tap outside it (unreachable with the margin) fails the call with AMB_ERR_UNSUPPORTED instead of reading past
+ * it.  A device band is read in place with no window: a raster that misses the stripe costs one launch, writes nothing
+ * and returns AMB_OK.
+ * Out of scope: datum shifts; geoid to ellipsoid heights (heights are imported as stored: SRTM and Copernicus heights
+ * are geoid heights); wrapping across the antimeridian (longitudes past +-180 are not folded); polar (UPS) maps.  With a
+ * host band or a TIFF, a map with a boundary cell whose position is not finite returns AMB_ERR_INVALID_ARGUMENT.
+ * Arguments and results as amb_import_raster / amb_import_raster_device / amb_import_tiff / amb_multi_import_*, plus
+ * map_epsg. */
+int amb_import_raster_lonlat(amb_ctx* ctx, int layer, const float* host_band, int32_t width, int32_t height,
+                             size_t row_stride, const double gt[6], int has_nodata, float nodata, int resample,
+                             int32_t map_epsg);
+int amb_import_raster_lonlat_device(amb_ctx* ctx, int layer, const float* device_band, int32_t width, int32_t height,
+                                    size_t row_stride, const double gt[6], int has_nodata, float nodata, int resample,
+                                    int32_t map_epsg);
+int amb_multi_import_raster_lonlat(amb_multi* m, int layer, const float* host_band, int32_t width, int32_t height,
+                                   size_t row_stride, const double gt[6], int has_nodata, float nodata, int resample,
+                                   int32_t map_epsg);
+int amb_import_tiff_lonlat(amb_ctx* ctx, int layer, const void* file, size_t bytes, const amb_tiff_layout* layout,
+                           const double gt[6], int has_nodata, float nodata, int resample, int32_t map_epsg);
+int amb_multi_import_tiff_lonlat(amb_multi* m, int layer, const void* file, size_t bytes, const amb_tiff_layout* layout,
+                                 const double gt[6], int has_nodata, float nodata, int resample, int32_t map_epsg);
+/* Host arithmetic, no GPU: the window {c_lo, c_hi, r_lo, r_hi} (inclusive) of a width x height raster that the stripe
+ * [col_begin, col_end) of `geom` reads, or {-1, -1, -1, -1} if the raster misses it.  What the imports above copy. */
+int amb_lonlat_import_window(const amb_geometry* geom, int32_t col_begin, int32_t col_end, int32_t map_epsg,
+                             int32_t width, int32_t height, const double gt[6], int32_t window[4]);
+/* Test hook: (lon, lat) in degrees of every cell of the context's stripe, d_lonlat[2 ((j - col_begin) rows + i)] and
+ * [.. + 1] (column-major like a layer), 8-byte-aligned device memory, computed by the device function the imports call;
+ * asynchronous on the context's stream. */
+int amb_lonlat_positions_device(amb_ctx* ctx, int32_t map_epsg, double* d_lonlat);
+
 /* ---- baseline JPEG of an 8-bit raster ----
  * Convention.  The file is byte for byte what libjpeg(-turbo) writes (OpenCV cv2.imencode(".jpg", img, params)) for the
  * same image with its defaults: SOI; APP0 JFIF 1.01, density 1:1 without units; one DQT per table; SOF0 (baseline,
